@@ -46,11 +46,11 @@ def measured_peaks():
             return json.load(open(p)), "measured"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": 3350.0}, "fallback (H100 SXM data sheet)"
 
 
 class ClockSampler:
-    """nvidia-smi samples DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi samples of SM clock, power and throttle reasons DURING the timed region."""
 
     def __init__(self, device):
         self.rows, self.proc, self.device = [], None, device
@@ -193,10 +193,12 @@ def run_ours(args):
     barrier(dist, local)
     ctx.timer_start()
     for _ in range(K):
-        step()
+        last = step()
     ms = ctx.timer_stop()
     ms = barrier_max(dist, local, ms)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:          # before any further step: the factor cache is the one the last timed step left
+        dump_outputs(args.dump_outputs, last, *f.read_back())
     launches = ctx.launches - launches0
     value = world * K / (ms * 1e-3)
 
@@ -243,7 +245,7 @@ def run_ours(args):
 
     # ---- roofline (HBM) for the kernels of the hot path; algorithmic bytes per SURVEY.md §8(d)
     peaks, src = measured_peaks()
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
     fp64_peak = ctx.fp64_tflops()
     kv = E / max(V, 1)
 
@@ -252,7 +254,7 @@ def run_ours(args):
         if t <= 0:
             return None
         r = {"kernel": "+".join(names), "bound": "hbm", "achieved": bytes_per_launch / (t * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s", "frac": bytes_per_launch / (t * 1e-3) / 1e9 / hbm,
-             "traffic": None, "ms": t, "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({src})", "algorithmic_bytes": bytes_per_launch}
+             "ms": t, "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({src})", "algorithmic_bytes": bytes_per_launch}
         if flops:
             r["fp64"] = {"achieved_tflops": flops / (t * 1e-3) / 1e12, "peak_tflops": fp64_peak, "frac": flops / (t * 1e-3) / 1e12 / fp64_peak, "peak_source": "vxs_diag_fp64_tflops (measured here)"}
         return r
@@ -279,16 +281,11 @@ def run_ours(args):
         t_sy = kern["k_syrk"]["ms_per_step"] * 1e-3 / max(kern["k_syrk"]["launches_per_step"], 1.0)
         fl_sy = V * 108.0 * kv * kv / max(kern["k_syrk"]["launches_per_step"], 1.0)      # 3 rank-1 rows x (6k)^2 / 2 MACs per voxel
         roof_main = {"kernel": "k_syrk", "bound": "tensor", "achieved": fl_sy / t_sy / 1e12, "peak": dmma_peak, "unit": "TFLOP/s", "frac": fl_sy / t_sy / 1e12 / dmma_peak,
-                     "traffic": ncu_traffic(["k_syrk"]), "peak_source": "vxs_diag_dmma_tflops: mma.sync.m8n8k4.f64 (SASS DMMA) throughput measured in this process; "
+                     "peak_source": "vxs_diag_dmma_tflops: mma.sync.m8n8k4.f64 (SASS DMMA) throughput measured in this process; "
                      "MEASURED_PEAKS.json carries no fp64 figure", "algorithmic_flops": fl_sy, "us_per_launch": t_sy * 1e6,
-                     "traffic_source": "profiles/r02_ncu_full_ba_kernels.txt (ncu --set full of this command, DRAM read + write per launch)",
                      "hbm_view_of_hessian_build": roof_hess,
                      "note": "the dominant kernel of the step is compute-bound on the fp64 tensor path; the HBM fractions the north_star names for the residual / Jacobian kernels are the "
                              "`roofline_residual` and `roofline_jac` keys of this line"}
-    for r_, names_ in ((roof_hess, ["k_jac_slab", "k_syrk"]), (roof_resid, resid_names), (roof_jac, ["k_jac_slab"])):
-        if r_ is not None:
-            r_["traffic"] = ncu_traffic(names_)
-            r_["traffic_source"] = "profiles/r02_ncu_full_ba_kernels.txt (ncu --set full of this command, DRAM read + write per launch)"
     dom = max(kern.items(), key=lambda kv_: kv_[1]["ms_per_step"])[0] if kern else None
 
     c2 = ds = None
@@ -333,7 +330,7 @@ def run_ours(args):
             "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic (seeded 3-plane room, SURVEY.md §8d; random-free IMU stand-in on the CPU callback)",
             "config": {"workload": f"metric shape M: W={W} window, {pts} pts/scan, L={L} m room, voxel 1 m, max_layer 2 -> V={V} plane voxels, E={E} (voxel,frame) clusters; n=15W={n} LI-BA system",
                        "step": "one LM iteration = vxs_li_ba(max_iter=1): Hessian build + IMU blocks (CPU callback) + damped LDLT + retraction + residual evaluation",
-                       "l2": "working set (clusters 80 B x E + rank-3 rows 144 B x V x W) is larger than the 126 MB L2; no extra flush",
+                       "l2": "working set (clusters 80 B x E + rank-3 rows 144 B x V x W) is larger than the 50 MB L2 of the H100; no extra flush",
                        "parallelism": "replicas: one independent window per GPU, no collective" if world > 1 else "1 GPU"},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h), "iterations_per_call": it_call,
                     "call": "vxs_factor_push_voxels_async of the host LidarFactor (pinned CSR, 4 chunks overlapped with the first Hessian build) + LI_BA damping_iter (3 iterations) + read back poses, Hessian, eig/pcr_adds"},
@@ -606,26 +603,21 @@ def gba_sharded_leg(vx, local, rank, world, dist, args):
     return res
 
 
-def ncu_traffic(kernels):
-    """DRAM bytes per launch (read + write) of the named kernels from the committed `ncu --set full` summary of this same command
-    (profiles/r02_ncu_full_ba_kernels.txt); None when the summary is absent."""
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r02_ncu_full_ba_kernels.txt")
-    try:
-        txt = open(path).read()
-    except OSError:
-        return None
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    total, seen = 0.0, set()
-    for blk in txt.split("== ")[1:]:
-        name = blk.split()[0]
-        if name not in kernels or name in seen:
-            continue
-        seen.add(name)
-        for line in blk.splitlines():
-            f = line.split()
-            if len(f) >= 3 and f[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                total += float(f[1]) * unit.get(f[2], 1.0)
-    return total if len(seen) == len(set(kernels)) else None
+def dump_outputs(d, o, eig, s, budget=64 << 20):
+    """What the timed step computed in its last run, as float64 .npy files under d: the vxs_li_ba results (states, residuals, LM trace) and the
+    factor cache it leaves behind (eig / pcr_adds of every voxel, read back as vxs_factor_read_back returns it).  Above `budget` bytes the factor
+    arrays keep a fixed, seeded sample of voxels (factor_rows.npy holds their indices)."""
+    os.makedirs(d, exist_ok=True)
+    tr = o["trace"]
+    out = {"states": o["states"], "resis": o["resis"], **{f"trace_{k}": tr[k] for k in ("r1", "r2", "u", "v", "q1", "accepted")}}
+    V = eig.shape[0]
+    keep = min(V, max(1, (budget - (1 << 20)) // ((eig.shape[1] + s.shape[1] + 1) * 8)))
+    if keep < V:
+        rows = np.sort(np.random.default_rng(0).choice(V, keep, replace=False))
+        eig, s, out["factor_rows"] = eig[rows], s[rows], rows
+    out["factor_eig12"], out["factor_sum10"] = eig, s
+    for k, v in out.items():
+        np.save(os.path.join(d, k + ".npy"), np.ascontiguousarray(v, dtype=np.float64))
 
 
 def ds_leg(ctx):
@@ -720,6 +712,8 @@ def cpu_baseline_from_structure(vx, W, ptr, fr, cl, eig, s, st0, tr, reps=2):
             out["reference_sources"] = {"value": 1.0 / min(tr_), "unit": UNIT, "cores": 5, "kind": "reference", "iterations_per_call": iters,
                                         "sample": "the reference's LI_BA_Optimizer::damping_iter (voxel_map.hpp compiled unmodified against the stand-in Eigen: scalar loops, no SSE packet "
                                                   "math; real IMU_PRE objects) on the same factor, best of 2 calls, call time / iterations executed"}
+        else:
+            out["reference_sources"] = {"error": "oracle/_ref/libvxref.so not built (needs the reference sources at build time)"}
     except Exception as e:          # noqa: BLE001 — the extra figure must never cost the bench line
         out["reference_sources"] = {"error": repr(e)}
     return out
@@ -982,7 +976,11 @@ def main():
     ap.add_argument("--gba-pts", type=int, default=50000)
     ap.add_argument("--gba-per-row", type=int, default=20)
     ap.add_argument("--gba-voxel", type=float, default=1.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (local-BA workload) to DIR/<name>.npy, float64, at most 64 MB")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "local_ba" or args.impl != "ours" or args.steps < 1):
+        ap.error("--dump-outputs writes what the timed local-BA step computed: it needs --workload local_ba, --impl ours and --steps >= 1")
     if args.workload == "hba":     # the hierarchical global-BA leg alone (same JSON block as the `gba` key of the default run)
         import voxel_slam_b200 as vx
         rank, world, local, dist = dist_setup(args)

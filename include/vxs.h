@@ -1,8 +1,8 @@
-/* vxs.h — C-ABI of the B200-native Voxel-SLAM bundle-adjustment hot path (libvxs.so).
+/* vxs.h — C-ABI of the H100-native Voxel-SLAM bundle-adjustment hot path (libvxs.so).
  *
  * The reference (hku-mars/Voxel-SLAM, one ROS C++ executable) has no plugin/FFI layer: the boundary of this path is
  * the C++ call surface used by VoxelSLAM/src/voxelslam.cpp.  Every entry point below names the reference interface it
- * replaces (file:line into /root/reference/VoxelSLAM/src/).  A header-only C++ shim with the reference's class names
+ * replaces (file:line into Voxel-SLAM/VoxelSLAM/src/).  A header-only C++ shim with the reference's class names
  * on top of this ABI is in voxel_slam_b200/csrc/shim/voxel_ba_shim.hpp; INTEGRATION.md shows the binding.
  *
  * Conventions

@@ -1,5 +1,5 @@
 // REFERENCE BUILD — TEST INFRASTRUCTURE ONLY.  This translation unit #includes the reference's OWN hot-path sources where they lie
-// (/root/reference/VoxelSLAM/src/{tools,preintegration,voxel_map,loop_refine}.hpp, unmodified, never copied into this repository) and exposes
+// (Voxel-SLAM/VoxelSLAM/src/{tools,preintegration,voxel_map,loop_refine}.hpp, unmodified, never copied into this repository) and exposes
 // them through the same C entry points as the hand-written oracle (vxo_capi.cpp, prefix vxr_ instead of vxo_), so that the oracle can be
 // pinned against the reference's real control flow, constants and formulas (tests/test_ref_pin.py) and the CUDA path can be checked against
 // the reference directly (tests/test_gpu_ref.py).  Eigen / PCL / ROS / GTSAM are absent from this image: they are replaced by the stand-in
@@ -17,7 +17,7 @@
 #include <cstring>
 #include <deque>
 #include "../include/vxs.h"
-#include "voxel_map.hpp"      // -I /root/reference/VoxelSLAM/src  (pulls tools.hpp, preintegration.hpp)
+#include "voxel_map.hpp"      // -I $VXS_REFERENCE_SRC  (pulls tools.hpp, preintegration.hpp)
 #include "loop_refine.hpp"
 #include "../tests/harness/synth.hpp"   // the seeded IMU sample generator shared with the harness (so both arms integrate the same samples)
 #ifndef DEG2RAD

@@ -8,7 +8,7 @@
 // finite-difference checks, numpy.linalg.eigh / scipy cross-checks and metamorphic properties
 // (tests/test_oracle_*.py).
 //
-// Restates (file:line are into /root/reference/VoxelSLAM/src/):
+// Restates (file:line are into Voxel-SLAM/VoxelSLAM/src/):
 //   tools.hpp:51-66      Exp            -> so3_exp
 //   tools.hpp:304-365    PointCluster   -> PC (push / cov / += / -= / transform)
 //   voxel_map.hpp:109-290  LidarFactor  -> LidarFactor (push_voxel, acc_evaluate2, evaluate_only_residual)

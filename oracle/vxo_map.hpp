@@ -1,6 +1,6 @@
 // ORACLE — TEST INFRASTRUCTURE ONLY (see vxo_core.hpp header; parity unpinned).
 //
-// Voxel-map side of the hot path, restated from /root/reference/VoxelSLAM/src/:
+// Voxel-map side of the hot path, restated from Voxel-SLAM/VoxelSLAM/src/:
 //   voxel_map.hpp:1511-1518 (= loop_refine.hpp:452-459)  float quantisation      -> voxel_key
 //   tools.hpp:24-49          VOXEL_LOC + hash                                    -> VoxelLoc, voxel_hash
 //   voxel_map.hpp:896-930    SlideWindow

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Golden vectors FROM THE REFERENCE'S OWN CODE.  Runs oracle/_ref/libvxref.so (the reference's hot-path sources compiled where they lie under
-/root/reference, see oracle/Makefile) on small seeded inputs and writes its outputs to tests/golden/reference_outputs.json.  The inputs are not
+VXS_REFERENCE_SRC, see oracle/Makefile) on small seeded inputs and writes its outputs to tests/golden/reference_outputs.json.  The inputs are not
 stored: they come from the seeded generators of tests/synth.py / tests/scenes.py, which travel with the repo, so tests/test_oracle_reference_golden.py
-can re-create them anywhere (the GPU box and any checkout without /root/reference included) and hold the hand-written oracle against these vectors.
+can re-create them anywhere (any checkout without the reference sources included) and hold the hand-written oracle against these vectors.
 
-    python tests/golden/make_reference_golden.py        (needs oracle/_ref/libvxref.so, i.e. this container)
+    python tests/golden/make_reference_golden.py        (needs oracle/_ref/libvxref.so)
 
 Floats are written as C99 hex strings (exact)."""
 import json
@@ -26,8 +26,8 @@ def hx(a):
 
 def main():
     if not ra.available():
-        sys.exit("oracle/_ref/libvxref.so is not built (needs /root/reference): run `make -C oracle ref` in the build container")
-    out = {"generator": "tests/golden/make_reference_golden.py", "source": "oracle/_ref/libvxref.so = /root/reference/VoxelSLAM/src/{tools,preintegration,voxel_map,loop_refine}.hpp + "
+        sys.exit("oracle/_ref/libvxref.so is not built: run `make -C oracle ref` (VXS_REFERENCE_SRC = the reference's VoxelSLAM/src)")
+    out = {"generator": "tests/golden/make_reference_golden.py", "source": "oracle/_ref/libvxref.so = Voxel-SLAM/VoxelSLAM/src/{tools,preintegration,voxel_map,loop_refine}.hpp + "
            "cut-outs of voxelslam.hpp / voxelslam.cpp, compiled unmodified against oracle/ref_standin", "cases": {}}
     c = out["cases"]
     # ---- a: a small window, from-scratch map build (cut_voxel + recut + tras_opt)

@@ -1,4 +1,4 @@
-"""The reference's own sources (oracle/_ref/libvxref.so, built by oracle/Makefile from /root/reference against the stand-in headers) behind the
+"""The reference's own sources (oracle/_ref/libvxref.so, built by oracle/Makefile from the reference sources at VXS_REFERENCE_SRC (see oracle/Makefile) against the stand-in headers) behind the
 same Python wrappers as the hand-written oracle: this module is tests/oracle_api.py executed a second time with BACKEND = "ref"."""
 import os as _os
 

@@ -112,14 +112,14 @@ def test_cpp_shim_typed_layer_type_checks_against_reference_signatures():
 
 def test_cpp_shim_typed_layer_compiles_against_the_reference_headers():
     """The typed layer against the reference's REAL tools.hpp / preintegration.hpp / voxel_map.hpp (IMUST, PointCluster, IMU_PRE, pointVar,
-    SlideWindow, Keyframe, PLV ...), with the stand-in Eigen / PCL / ROS headers of oracle/ref_standin; skipped where /root/reference is absent
+    SlideWindow, Keyframe, PLV ...), with the stand-in Eigen / PCL / ROS headers of oracle/ref_standin; skipped where the reference's VoxelSLAM/src (VXS_REFERENCE_SRC, default as in oracle/Makefile) is absent
     (the stub-based check above still runs there).  Also checks the layout assumptions (sizeof(pointVar), sizeof(PointType))."""
     import subprocess
     import tempfile
     import pytest
-    ref = "/root/reference/VoxelSLAM/src"
+    ref = os.environ.get("VXS_REFERENCE_SRC", "/root/reference/VoxelSLAM/src")      # same default as oracle/Makefile
     if not os.path.exists(os.path.join(ref, "voxel_map.hpp")):
-        pytest.skip("reference sources not present on this box")
+        pytest.skip("reference sources (VXS_REFERENCE_SRC) not present")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     src = '#include "voxel_map.hpp"\nstatic_assert(sizeof(pointVar) == 96 && sizeof(PointType) == 48, "record layouts the C-ABI relies on");\n' + SHIM_USE
     with tempfile.NamedTemporaryFile("w", suffix=".cpp", delete=False) as f:

@@ -33,7 +33,7 @@ def test_cpu_baseline_from_structure_runs_on_host():
     assert out["first_iteration"]["r1"] > 0
     import ref_api as ra
     rs = out["reference_sources"]
-    if ra.available():          # oracle/_ref is built wherever /root/reference exists; on a box without it the leg must say so, not crash
+    if ra.available():          # oracle/_ref is built where the reference sources exist (VXS_REFERENCE_SRC); on a box without it the leg must say so, not crash
         assert "error" not in rs, rs
         assert rs["kind"] == "reference" and rs["value"] > 0 and 1 <= rs["iterations_per_call"] <= 3
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): CUDA path through the C-ABI vs the CPU oracle on the same seeded inputs.
+"""GPU parity tests (run on an H100): CUDA path through the C-ABI vs the CPU oracle on the same seeded inputs.
 Tolerances: BASELINE.json asks for 1e-5 relative on residuals / H / g / pose increments; the kernels are fp64 and are held
 to far tighter bounds here (stated per assert)."""
 import threading

@@ -1,6 +1,6 @@
 """Multi-GPU parity of the voxel-sharded global-BA step under pytest -m gpu: launches tests/multi_gpu_worker.py with torchrun on 2 GPUs
 (sharded LM solve, an empty shard, sharded HBA window — each compared with the single-process oracle inside the worker).
-Skipped on a box with fewer than 2 GPUs (the driver's 1-GPU test tier); `gpurun --gpus 2 -- python -m pytest tests -m gpu` runs it."""
+Skipped on a machine with fewer than 2 GPUs; `python -m pytest tests -m gpu` on a multi-GPU machine runs it."""
 import os
 import subprocess
 import sys

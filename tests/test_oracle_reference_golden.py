@@ -1,6 +1,6 @@
 """The oracle against GOLDEN VECTORS PRODUCED BY THE REFERENCE'S OWN CODE (tests/golden/reference_outputs.json, written by
 tests/golden/make_reference_golden.py from oracle/_ref/libvxref.so in the build container).  Unlike tests/test_ref_pin.py this needs neither
-/root/reference nor the reference build: the inputs are re-created from the seeded harness generators (tests/golden_cases.py), so the pin holds on the
+the reference sources nor the reference build: the inputs are re-created from the seeded harness generators (tests/golden_cases.py), so the pin holds on the
 GPU box and in any checkout.  Tolerances are those of test_ref_pin.py (what is left is Eigen-internal summation order)."""
 import json
 import os

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise ncu outputs into small text files for profiles/.
+"""Summarise ncu outputs into small text files.
   python tools/ncu_summary.py launches gpurun_out/launches.csv            -> per-kernel count / total / share
   python tools/ncu_summary.py full gpurun_out/prof.ncu-rep                -> key counters per captured kernel (needs ncu here)
 """

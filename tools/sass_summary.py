@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Static SASS evidence for profiles/: per-kernel counts of the mnemonics that show which hardware paths libvxs.so uses
+"""Static SASS evidence: per-kernel counts of the mnemonics that show which hardware paths libvxs.so uses
 (DMMA = mma.sync.m8n8k4.f64, UBLKCP = cp.async.bulk, SYNCS = mbarrier, LDGSTS = cp.async, RED/ATOM .F64).  No GPU needed:
-    python tools/sass_summary.py > profiles/r02_sass_summary.txt"""
+    python tools/sass_summary.py"""
 import collections
 import os
 import re
@@ -44,7 +44,7 @@ def main():
     keys = list(PAT)
     print(f"SASS mnemonic counts per kernel of voxel_slam_b200/lib/libvxs.so (cuobjdump -sass; cubin arch {sorted(arch)}; STATIC instruction counts, not executed counts)")
     print("produced by tools/sass_summary.py.  DMMA = mma.sync.m8n8k4.f64 (fp64 tensor path), UBLKCP = cp.async.bulk (1-D TMA), SYNCS = mbarrier ops, LDGSTS = cp.async,")
-    print("RED.F64 = fp64 reduction atomics.  tcgen05 / TMEM have no fp64 kind, so no UTC* instructions are expected in this library.\n")
+    print("RED.F64 = fp64 reduction atomics.\n")
     print("%-44s %7s " % ("kernel", "instrs") + " ".join("%7s" % k for k in keys))
     tot = collections.Counter()
     for d, n, c in rows:

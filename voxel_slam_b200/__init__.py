@@ -1,4 +1,4 @@
-"""voxel_slam_b200 — B200-native (sm_100a CUDA) bundle-adjustment hot path of hku-mars/Voxel-SLAM.
+"""voxel_slam_b200 — H100-native (sm_90a CUDA) bundle-adjustment hot path of hku-mars/Voxel-SLAM.
 
 The product is the C-ABI shared library ``lib/libvxs.so`` (``include/vxs.h``); this package is the thin Python
 mirror used by the tests and ``bench.py``.  There is no CPU fallback: importing works anywhere (so that the

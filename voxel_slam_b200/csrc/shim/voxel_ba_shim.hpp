@@ -10,7 +10,7 @@
 //   * a plain layer (no Eigen): flat arrays in, flat arrays out — compile-tested in this repository (tests/test_abi.py);
 //   * an Eigen/reference-typed layer behind VXS_SHIM_WITH_REFERENCE_TYPES: include it AFTER the reference's tools.hpp, preintegration.hpp and
 //     voxel_map.hpp (it uses their IMUST, PointCluster, IMU_PRE, DIM, pointVar, PVecPtr, SlideWindow, Keyframe).  tests/test_abi.py compiles
-//     this layer against the reference's REAL headers from /root/reference (with stand-in headers for the Eigen / PCL /
+//     this layer against the reference's REAL headers from the reference checkout (with stand-in headers for the Eigen / PCL /
 //     ROS headers this image lacks) and, on boxes without the reference, against tests/shim_stubs/reference_stubs.hpp.
 #pragma once
 #include <cstring>

@@ -1,4 +1,4 @@
-// LidarFactor evaluation kernels (sm_100a): evaluate_only_residual and acc_evaluate2 of the reference
+// LidarFactor evaluation kernels (sm_90a): evaluate_only_residual and acc_evaluate2 of the reference
 // (voxel_map.hpp:243-279, 132-241), re-designed for the GPU:
 //
 //   k_cluster_sum   sub-warp group per voxel, lanes over the voxel's CSR entries; coalesced SoA fp64 loads of the clusters,
@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(256) k_cluster_sum(FactorView f, const double*
       cluster_transform_acc(c, R, t, acc);
     }
     if (G == 32) {
-      // reduce-scatter over the warp: 12 64-bit shuffles instead of 50 (the kernel was LSU-bound on shuffles, profiles/):
+      // reduce-scatter over the warp: 12 64-bit shuffles instead of 50 (the kernel was LSU-bound on shuffles):
       // after the five steps the lanes with even index hold one fully reduced component each.
       double a[10] = {acc.P.xx, acc.P.xy, acc.P.xz, acc.P.yy, acc.P.yz, acc.P.zz, acc.v.x, acc.v.y, acc.v.z, acc.n};
       const bool b16 = lane & 16, b8 = lane & 8, b4 = lane & 4, b2 = lane & 2;
@@ -422,10 +422,9 @@ __global__ void __launch_bounds__(256) k_bd_zero(double* __restrict__ Cbd, doubl
 }
 
 // ------------------------------------------------------------------ Hessian part 2b: dense windows, SYRK on the fp64 tensor cores
-// H -= X^T X with X = (3V) x (6W).  Measured on B200 (profiles/): with scalar DFMA the kernel is limited by the
-// shared-memory -> register delivery (2 B per FMA at 72 accumulators/thread equals the 128 B/clk LSU limit at full FP64 rate),
-// not by the FP64 pipe.  mma.sync.m8n8k4.f64 (SASS DMMA, same 36.9 TFLOP/s peak as the FMA pipe on B200) shares each operand
-// across 8 lanes inside the tensor core: 0.33 B per FMA.
+// H -= X^T X with X = (3V) x (6W).  With scalar DFMA the kernel is limited by the shared-memory -> register delivery
+// (2 B per FMA at 72 accumulators/thread equals the 128 B/clk LSU limit at full FP64 rate), not by the FP64 pipe.
+// mma.sync.m8n8k4.f64 (SASS DMMA, Hopper's fp64 tensor path) shares each operand across 8 lanes inside the tensor core: 0.33 B per FMA.
 //   * column blocks of 8 frames (48 columns), the remainder block (W mod 8 frames) FIRST so it only pairs with itself;
 //   * warp unit = (row block a, column block b), a <= b: 6x6 mma tiles of 8x8, 72 fp64 accumulators per lane;
 //   * CTA = 2x2 units; k runs over (voxel, m) rows in chunks of 4; XT (see xt_index) is staged with 16-B cp.async,

@@ -7,7 +7,7 @@
 #include <vector>
 #include "../../include/vxs.h"
 
-#define VXS_SM_COUNT_FALLBACK 148
+#define VXS_SM_COUNT_FALLBACK 132
 
 struct vxs_stage {
   const char* name;

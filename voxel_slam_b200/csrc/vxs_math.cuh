@@ -1,7 +1,7 @@
 // Per-voxel / per-entry math of the BA hot path, written for the GPU (register-resident fp64, no local arrays
 // with dynamic indexing) but compilable as plain C++ so tests can exercise it on the CPU (tests/test_host_math.py).
 //
-// What it restates (reference = /root/reference/VoxelSLAM/src/):
+// What it restates (reference = Voxel-SLAM/VoxelSLAM/src/):
 //   tools.hpp:357-363        PointCluster::transform            -> cluster_transform_acc
 //   voxel_map.hpp:264-273    cov + SelfAdjointEigenSolver        -> cov_from_sum, eig3_jacobi
 //   voxel_map.hpp:163-234    acc_evaluate2 per observing frame   -> entry_jacobian  (rank-3 + block-diagonal form,

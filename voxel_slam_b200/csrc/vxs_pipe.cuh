@@ -1,4 +1,4 @@
-// mbarrier + bulk-copy (TMA 1-D, cp.async.bulk) helpers for the producer / consumer pipelines of the streaming kernels (sm_100a).
+// mbarrier + bulk-copy (TMA 1-D, cp.async.bulk) helpers for the producer / consumer pipelines of the streaming kernels (sm_90a).
 //   producer (one elected lane): wait empty[s] -> arrive.expect_tx full[s] -> cp.async.bulk ... complete_tx on full[s]
 //   consumers                  : wait full[s] -> use the stage -> (fence.proxy.async if they wrote it) -> one arrive per warp on empty[s]
 // A CTA that is not part of a cluster launch is a cluster of one, so the .shared::cluster destination of the bulk copy is its own

@@ -1,4 +1,4 @@
-// evaluate_only_residual (voxel_map.hpp:243-279) as ONE streaming kernel (sm_100a):
+// evaluate_only_residual (voxel_map.hpp:243-279) as ONE streaming kernel (sm_90a):
 //
 //   k_residual_stream   persistent, per_sm CTAs per SM (default: 3 CTAs of TE = 256 consumer threads + one producer warp, 2 stages each; tuned on the
 //                       metric shape, see launch_resid).  The producer warp streams the SoA cluster columns (80 B per (voxel, frame) entry, + the
