@@ -59,8 +59,10 @@ int vxs_ctx_timer_stop(vxs_ctx* ctx, double* ms);
 /* diagnostics: measured fp64 FMA throughput of this device (TFLOP/s, 2 flop per FMA) — the roofline denominator of the
  * SYRK part of the Hessian, which MEASURED_PEAKS.json does not carry */
 int vxs_diag_fp64_tflops(vxs_ctx* ctx, double* tflops);
-/* same for the fp64 tensor-core path (mma.sync.m8n8k4.f64, SASS DMMA) */
+/* same for the fp64 tensor-core path, in the MMA shape the SYRK issues (mma.sync.m16n8k4.f64, SASS DMMA.16x8x4) */
 int vxs_diag_dmma_tflops(vxs_ctx* ctx, double* tflops);
+/* measured throughput (TFLOP/s) of each fp64 mma.sync shape: tflops[0..3] = m8n8k4, m16n8k4, m16n8k8, m16n8k16 */
+int vxs_diag_dmma_shapes(vxs_ctx* ctx, double tflops[4]);
 /* damped solve of a synthetic n x n system: out[0] = ms per solve (events), out[1..4] = us per 32-column panel that CTA 0 spends in
  * {panel load, strip solve, Schur update, grid barrier}, out[5] = panels, out[6] = SM clock (kHz) used for the conversion,
  * out[7] = us per panel of the look-ahead diagonal factor, out[8] = residual |(H + u diag H) dx + g|_inf / |g|_inf of the solve

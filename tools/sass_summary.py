@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Static SASS evidence: per-kernel counts of the mnemonics that show which hardware paths libvxs.so uses
-(DMMA = mma.sync.m8n8k4.f64, UBLKCP = cp.async.bulk, SYNCS = mbarrier, LDGSTS = cp.async, RED/ATOM .F64).  No GPU needed:
+(DMMA16 = mma.sync.m16n8k{4,8,16}.f64, DMMA8 = mma.sync.m8n8k4.f64, UBLKCP = cp.async.bulk, SYNCS = mbarrier, LDGSTS = cp.async, RED/ATOM .F64).  No GPU needed:
     python tools/sass_summary.py"""
 import collections
 import os
@@ -10,7 +10,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "voxel_slam_b200", "lib", "libvxs.so")
-PAT = {"DMMA": r"\bDMMA", "UBLKCP": r"UBLKCP", "SYNCS": r"\bSYNCS", "LDGSTS": r"LDGSTS", "RED.F64": r"(RED|REDG|ATOM|ATOMG)\.E\.ADD\.F64", "BAR": r"\bBAR\.", "DFMA": r"\bDFMA",
+PAT = {"DMMA16": r"\bDMMA\.16x8x", "DMMA8": r"\bDMMA\.8x8x4", "UBLKCP": r"UBLKCP", "SYNCS": r"\bSYNCS", "LDGSTS": r"LDGSTS", "RED.F64": r"(RED|REDG|ATOM|ATOMG)\.E\.ADD\.F64", "BAR": r"\bBAR\.", "DFMA": r"\bDFMA",
        "LDG": r"\bLDG", "STG": r"\bSTG", "LDS": r"\bLDS", "STS": r"\bSTS"}
 
 
@@ -43,7 +43,8 @@ def main():
     rows.sort(key=lambda r: -r[1])
     keys = list(PAT)
     print(f"SASS mnemonic counts per kernel of voxel_slam_b200/lib/libvxs.so (cuobjdump -sass; cubin arch {sorted(arch)}; STATIC instruction counts, not executed counts)")
-    print("produced by tools/sass_summary.py.  DMMA = mma.sync.m8n8k4.f64 (fp64 tensor path), UBLKCP = cp.async.bulk (1-D TMA), SYNCS = mbarrier ops, LDGSTS = cp.async,")
+    print("produced by tools/sass_summary.py.  DMMA16 = mma.sync.m16n8k{4,8,16}.f64 (Hopper fp64 tensor shapes), DMMA8 = mma.sync.m8n8k4.f64 (Ampere shape),\n"
+          "UBLKCP = cp.async.bulk (1-D TMA), SYNCS = mbarrier ops, LDGSTS = cp.async,")
     print("RED.F64 = fp64 reduction atomics.\n")
     print("%-44s %7s " % ("kernel", "instrs") + " ".join("%7s" % k for k in keys))
     tot = collections.Counter()

@@ -152,6 +152,14 @@ class Context:
         self._check(lib().vxs_diag_dmma_tflops(self._p, C.byref(t)))
         return t.value
 
+    DMMA_SHAPES = ("m8n8k4", "m16n8k4", "m16n8k8", "m16n8k16")
+
+    def dmma_shapes_tflops(self):
+        """Measured TFLOP/s of each fp64 mma.sync shape, as {shape: rate} in DMMA_SHAPES order."""
+        t = (C.c_double * 4)()
+        self._check(lib().vxs_diag_dmma_shapes(self._p, t))
+        return dict(zip(self.DMMA_SHAPES, list(t)))
+
     def ldlt_phases(self, n):
         out = (C.c_double * 12)()
         self._check(lib().vxs_diag_ldlt_phases(self._p, int(n), out))

@@ -30,7 +30,7 @@ extern "C" int vxs_ctx_create(int device, vxs_ctx** out) {
   c->scal.reserve(64);
   c->flags.reserve(16);
   { const char* e = getenv("VXS_LDLT_LOOKAHEAD_CTA"); c->ldlt_lookahead = (e && e[0] == '0') ? 0 : 1; }
-  { const char* e = getenv("VXS_SYRK_WAVES"); c->syrk_waves = e ? std::max(1, atoi(e)) : 12; }
+  { const char* e = getenv("VXS_SYRK_WAVES"); c->syrk_waves = e ? std::max(1, atoi(e)) : 8; }
   { const char* e = getenv("VXS_SYRK_ONLY_TILE"); c->syrk_only_tile = e ? atoi(e) : -1; }
   { const char* e = getenv("VXS_RESID_STREAM"); c->resid_stream = (e && e[0] == '0') ? 0 : 1; }
   { const char* e = getenv("VXS_RESID_TE"); if (e) c->resid_te = atoi(e); }
@@ -159,39 +159,75 @@ extern "C" int vxs_diag_fp64_tflops(vxs_ctx* c, double* tflops) {
   return VXS_OK;
 }
 
-// fp64 tensor-core (DMMA, mma.sync.m8n8k4.f64) peak: 8 independent accumulator tiles per warp
+// fp64 tensor-core (DMMA) peak of one mma.sync shape: 8 independent accumulator tiles per warp.
+// SHAPE 0 = m8n8k4 (Ampere's shape, SASS DMMA.8x8x4), 1 = m16n8k4, 2 = m16n8k8, 3 = m16n8k16 (Hopper, DMMA.16x8x{4,8,16}).
+constexpr int kDmmaShapes = 4;
+constexpr int dmma_shape_fma(int shape) { return shape == 0 ? 8 * 8 * 4 : 16 * 8 * (4 << (shape - 1)); }
+template <int SHAPE>
 __global__ void __launch_bounds__(256) k_dmma_peak(double* out, int iters) {
-  double c[16];
+  constexpr int NC = SHAPE == 0 ? 2 : 4;    // accumulator registers per tile
+  double c[8 * NC];
 #pragma unroll
-  for (int i = 0; i < 16; i++) c[i] = 0.0;
-  double a = 1.0 + threadIdx.x * 1e-9, b = 1.0 - threadIdx.x * 1e-9;
+  for (int i = 0; i < 8 * NC; i++) c[i] = 0.0;
+  double a[8], b[4];
+#pragma unroll
+  for (int i = 0; i < 8; i++) a[i] = 1.0 + (threadIdx.x + i) * 1e-9;
+#pragma unroll
+  for (int i = 0; i < 4; i++) b[i] = 1.0 - (threadIdx.x + i) * 1e-9;
   for (int it = 0; it < iters; it++) {
 #pragma unroll
-    for (int t = 0; t < 8; t++)
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c[2 * t]), "+d"(c[2 * t + 1]) : "d"(a), "d"(b));
+    for (int t = 0; t < 8; t++) {
+      double* d = c + NC * t;
+      if (SHAPE == 0)
+        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(d[0]), "+d"(d[1]) : "d"(a[0]), "d"(b[0]));
+      else if (SHAPE == 1)
+        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                     : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3]) : "d"(a[0]), "d"(a[1]), "d"(b[0]));
+      else if (SHAPE == 2)
+        asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                     : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+      else
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+                     : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
+    }
   }
   double s = 0;
 #pragma unroll
-  for (int i = 0; i < 16; i++) s += c[i];
+  for (int i = 0; i < 8 * NC; i++) s += c[i];
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
-extern "C" int vxs_diag_dmma_tflops(vxs_ctx* c, double* tflops) {
-  if (!c || !tflops) return VXS_ERR_ARG;
+// best of three timed launches after one warm-up; every shape does the same flops per launch
+static int dmma_shape_tflops(vxs_ctx* c, int shape, double* tflops) {
   cudaSetDevice(c->device);
-  const int blocks = c->sm_count * 4, iters = 4000;
+  const int blocks = c->sm_count * 4, iters = 4000 * dmma_shape_fma(0) / dmma_shape_fma(shape);
+  void (*const kernels[kDmmaShapes])(double*, int) = {k_dmma_peak<0>, k_dmma_peak<1>, k_dmma_peak<2>, k_dmma_peak<3>};
   VXS_CUDA(c, c->stage.reserve(size_t(blocks) * 256));
   double best = 0;
   for (int rep = 0; rep < 4; rep++) {
     VXS_CUDA(c, cudaEventRecord(c->ev_t0, c->stream));
-    VXS_LAUNCH(c, "k_dmma_peak", k_dmma_peak, blocks, 256, 0, c->stage.p, iters);
+    VXS_LAUNCH(c, "k_dmma_peak", kernels[shape], blocks, 256, 0, c->stage.p, iters);
     VXS_CUDA(c, cudaEventRecord(c->ev_t1, c->stream));
     VXS_CUDA(c, cudaEventSynchronize(c->ev_t1));
     float ms = 0;
     VXS_CUDA(c, cudaEventElapsedTime(&ms, c->ev_t0, c->ev_t1));
-    const double tf = double(blocks) * 8 /*warps*/ * iters * 8 /*mma*/ * 256 /*fma*/ * 2 / (ms * 1e-3) / 1e12;
+    const double tf = double(blocks) * 8 /*warps*/ * iters * 8 /*mma*/ * dmma_shape_fma(shape) * 2 / (ms * 1e-3) / 1e12;
     if (rep > 0 && tf > best) best = tf;
   }
   *tflops = best;
+  return VXS_OK;
+}
+// the shape k_syrk issues (m16n8k4), so that it is the ceiling of the kernel's own instruction
+extern "C" int vxs_diag_dmma_tflops(vxs_ctx* c, double* tflops) {
+  if (!c || !tflops) return VXS_ERR_ARG;
+  return dmma_shape_tflops(c, 1, tflops);
+}
+extern "C" int vxs_diag_dmma_shapes(vxs_ctx* c, double tflops[4]) {
+  if (!c || !tflops) return VXS_ERR_ARG;
+  for (int s = 0; s < kDmmaShapes; s++) {
+    int rc = dmma_shape_tflops(c, s, tflops + s);
+    if (rc) return rc;
+  }
   return VXS_OK;
 }
 

@@ -8,8 +8,8 @@
 //                   two-level reduction of sum coe*lambda0 ("last block" pattern).         176 B / voxel
 //   k_jac           group per voxel, lane per entry: g_i, D_i and the three scaled rank-1 rows x^m_i (SURVEY App. A.3),
 //                   rows stored for the SYRK, g/D accumulated with fp64 RED.                 k*80+176 B read, k*144 B written / voxel
-//   k_syrk          H -= X^T X on the fp64 tensor cores (mma.sync.m8n8k4.f64 / DMMA): warp unit = 48x48 output (8x8 frames,
-//                   6x6 mma tiles, 72 accumulators/lane), CTA = 2x2 units, X staged with cp.async (zero-fill), 3 stages;
+//   k_syrk          H -= X^T X on the fp64 tensor cores (mma.sync.m16n8k4.f64 / DMMA.16x8x4): warp unit = 48x48 output (8x8 frames,
+//                   6x6 tiles of 8x8, one MMA per pair of tile rows, 72 accumulators/lane), CTA = 2x2 units, X staged with cp.async (zero-fill), 3 stages;
 //                   split over voxel chunks, fp64 RED epilogue.  fp64-bound for k >~ 4 (SURVEY §7.3).
 //   k_pairs         sparse windows (k << W, top-level global BA): group per voxel, block pairs straight to RED.
 //   k_assemble      dense n x n system from the block accumulators (+ the CPU-evaluated IMU 30x30 blocks), mirror of the lower triangle.
@@ -424,9 +424,12 @@ __global__ void __launch_bounds__(256) k_bd_zero(double* __restrict__ Cbd, doubl
 // ------------------------------------------------------------------ Hessian part 2b: dense windows, SYRK on the fp64 tensor cores
 // H -= X^T X with X = (3V) x (6W).  With scalar DFMA the kernel is limited by the shared-memory -> register delivery
 // (2 B per FMA at 72 accumulators/thread equals the 128 B/clk LSU limit at full FP64 rate), not by the FP64 pipe.
-// mma.sync.m8n8k4.f64 (SASS DMMA, Hopper's fp64 tensor path) shares each operand across 8 lanes inside the tensor core: 0.33 B per FMA.
+// mma.sync.m16n8k4.f64 (SASS DMMA.16x8x4, one of Hopper's fp64 tensor shapes) shares each operand across 8 lanes inside the tensor core.
+// On an H100 80GB HBM3 (700 W power limit, 1980 MHz; tools/dmma_shapes.py) it runs at 66.5 TFLOP/s, twice Ampere's m8n8k4 (33.4);
+// m16n8k8 / m16n8k16 measure the same 66.3 / 66.2, so the SYRK uses the k4 shape, whose fragments are the ones the XT layout stages.
 //   * column blocks of 8 frames (48 columns), the remainder block (W mod 8 frames) FIRST so it only pairs with itself;
-//   * warp unit = (row block a, column block b), a <= b: 6x6 mma tiles of 8x8, 72 fp64 accumulators per lane;
+//   * warp unit = (row block a, column block b), a <= b: 6x6 tiles of 8x8, 72 fp64 accumulators per lane; one m16n8k4 covers the two
+//     tiles (ti = 0, 1) of a tile column inside a piece (see SyPiece), its A fragment is exactly the two 8-column runs the XT layout stages;
 //   * CTA = 2x2 units; k runs over (voxel, m) rows in chunks of 4; XT (see xt_index) is staged with 16-B cp.async,
 //     3 stages of 4 voxels (12 rows); split over voxel chunks; fp64 RED epilogue into the upper block triangle.
 #define SY_THREADS 128
@@ -443,8 +446,11 @@ __device__ __forceinline__ void cp_async16_zfill(void* smem_dst, const void* gsr
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+// C[16x8] += A[16x4] B[4x8] (SASS DMMA.16x8x4).  Lane (g = lane/4, t = lane%4) holds a0 = A[g][t], a1 = A[g+8][t], b = B[t][g],
+// c0, c1 = C[g][2t, 2t+1] and c2, c3 = C[g+8][2t, 2t+1].
+__device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+               : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3) : "d"(a0), "d"(a1), "d"(b));
 }
 
 struct SyrkGeom { int r0, ngc, nbp, ntiles; };
@@ -464,49 +470,120 @@ static SyrkGeom sy_geom(int W) {
 // the SM) busy on diagonal / remainder tiles, where a unit-per-warp mapping leaves one to three warps idle.
 struct SyPiece { int offI, offJ, ntI, ntJ, rowbase, colbase, nvalI, nvalJ; unsigned mask; };   // mask: bit ti*6+tj = tile needed
 
-__global__ void __launch_bounds__(SY_THREADS, 2) k_syrk(const double* __restrict__ XT, double* __restrict__ C, int g_first, int ngroups_vox, int W, SyrkGeom g, int groups_per_chunk, int only_tile) {
-  extern __shared__ __align__(16) double smem[];
-  const int tile = only_tile >= 0 ? only_tile : int(blockIdx.x % g.ntiles), chunk = only_tile >= 0 ? int(blockIdx.x) : int(blockIdx.x / g.ntiles);   // only_tile: diagnostic (cost of one tile kind)
-  int A = 0, rem = tile;
-  while (rem >= g.nbp - A) { rem -= g.nbp - A; A++; }
-  const int B = A + rem;
-  const int g_begin = g_first + chunk * groups_per_chunk, g_end = min(ngroups_vox, g_begin + groups_per_chunk);   // voxel groups [g_first, ngroups_vox)
-  if (g_begin >= g_end) return;
+// tile index -> (row part A, column part B), A <= B
+__host__ __device__ inline void sy_tile_parts(const SyrkGeom& g, int tile, int& A, int& B) {
+  int a = 0, rem = tile;
+  while (rem >= g.nbp - a) { rem -= g.nbp - a; a++; }
+  A = a; B = a + rem;
+}
+
+// The pieces of tile (A, B) that `warp` runs: the tile's pieces in a fixed order, piece q to warp q % 4 (warp-uniform, <= 3 per warp).
+// The stream-K cost model (sy_tile_cost) counts the same enumeration.
+__host__ __device__ inline int sy_pieces(const SyrkGeom& g, int A, int B, int warp, SyPiece (&pc)[3]) {
+  int npc = 0, q = 0;
+  for (int u = 0; u < 4; u++) {
+    const int wy = u >> 1, wx = u & 1, ga = 2 * A + wy, gb = 2 * B + wx;
+    if (!(ga < g.ngc && gb < g.ngc && ga <= gb)) continue;
+    const int nvalI = 6 * sy_glen(g, ga), nvalJ = 6 * sy_glen(g, gb);
+    const int ntI = (nvalI + 7) >> 3, ntJ = (nvalJ + 7) >> 3;
+    for (int t0 = 0; t0 < ntI; t0 += 2, q++) {
+      if ((q & 3) != warp || npc >= 3) continue;
+      SyPiece P;
+      P.offI = (wy ? 6 * sy_glen(g, 2 * A) : 0) + 8 * t0;
+      P.offJ = wx ? 6 * sy_glen(g, 2 * B) : 0;
+      P.ntI = ntI - t0 < 2 ? ntI - t0 : 2; P.ntJ = ntJ;
+      P.rowbase = 6 * sy_gstart(g, ga) + 8 * t0; P.colbase = 6 * sy_gstart(g, gb);
+      P.nvalI = nvalI - 8 * t0; P.nvalJ = nvalJ;
+      // tiles of a diagonal unit whose rows all belong to later frames than all of their columns hold only pairs with
+      // frame(i) > frame(j): never stored (11 of the 36 tiles of a full diagonal unit)
+      P.mask = 0u;
+      for (int ti = 0; ti < P.ntI; ti++)
+        for (int tj = 0; tj < P.ntJ; tj++)
+          if (!(ga == gb && (8 * (t0 + ti)) / 6 > (8 * tj + 7) / 6)) P.mask |= 1u << (ti * 6 + tj);
+      if (npc == 0) pc[0] = P; else if (npc == 1) pc[1] = P; else pc[2] = P;
+      npc++;
+    }
+  }
+  return npc;
+}
+
+// operand fragments of k-chunk kc of a piece (pI, pJ: the piece's row / column operands in the stage, lane offset included)
+__device__ __forceinline__ void sy_frags(const double* pI, const double* pJ, int kc, double (&fa)[2], double (&fb)[6]) {
+#pragma unroll
+  for (int t = 0; t < 2; t++) fa[t] = pI[(kc * SY_PCOLS + 8 * t) * 4];
+#pragma unroll
+  for (int t = 0; t < 6; t++) fb[t] = pJ[(kc * SY_PCOLS + 8 * t) * 4];
+}
+
+// One k-chunk (4 rows of X) of a piece: one m16n8k4 per tile column tj covers both tile rows ti = 0, 1 (acc[2tj..] and acc[12+2tj..]).
+// A column is skipped only when its ti = 0 tile is masked out: its ti = 1 tile (later frames) then is too.  A tile that is computed but
+// masked out (ti = 1 of a diagonal column, or the missing second tile row of a one-row piece) is never stored: sy_epilogue tests the mask.
+__device__ __forceinline__ void sy_mma_chunk(double* acc, unsigned mask, const double (&fa)[2], const double (&fb)[6]) {
+  if ((mask & 0x3Fu) == 0x3Fu) {
+#pragma unroll
+    for (int tj = 0; tj < 6; tj++) dmma1684(acc[2 * tj], acc[2 * tj + 1], acc[12 + 2 * tj], acc[13 + 2 * tj], fa[0], fa[1], fb[tj]);
+  } else {
+#pragma unroll
+    for (int tj = 0; tj < 6; tj++)
+      if ((mask >> tj) & 1u) dmma1684(acc[2 * tj], acc[2 * tj + 1], acc[12 + 2 * tj], acc[13 + 2 * tj], fa[0], fa[1], fb[tj]);
+  }
+}
+
+// all pieces of one staged voxel group (3 k-chunks)
+__device__ __forceinline__ void sy_stage_mma(double (&acc)[72], const SyPiece (&pc)[3], int npc, const double* sI, const double* sJ) {
+#pragma unroll
+  for (int p = 0; p < 3; p++) {
+    if (p < npc) {
+      const double* pI = sI + size_t(pc[p].offI) * 4;
+      const double* pJ = sJ + size_t(pc[p].offJ) * 4;
+#pragma unroll
+      for (int kc = 0; kc < 3; kc++) {
+        double fa[2], fb[6];
+        sy_frags(pI, pJ, kc, fa, fb);
+        sy_mma_chunk(acc + p * 24, pc[p].mask, fa, fb);
+      }
+    }
+  }
+}
+
+// lane holds C[8ti + lane/4][8tj + 2(lane%4) + {0,1}] of every tile of its pieces; H_ij -= x_i x_j^T for frame(i) <= frame(j), fp64 RED
+__device__ __forceinline__ void sy_epilogue(const double (&acc)[72], const SyPiece (&pc)[3], int npc, int lane, double* __restrict__ C, int n) {
+  const int rl = lane >> 2, cl = 2 * (lane & 3);
+#pragma unroll
+  for (int p = 0; p < 3; p++) {
+    if (p < npc) {
+#pragma unroll
+      for (int ti = 0; ti < 2; ti++)
+#pragma unroll
+        for (int tj = 0; tj < 6; tj++) {
+          const int r = 8 * ti + rl;
+          if (((pc[p].mask >> (ti * 6 + tj)) & 1u) && r < pc[p].nvalI) {
+            const int R = pc[p].rowbase + r;
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+              const int c = 8 * tj + cl + e;
+              const int Cc = pc[p].colbase + c;
+              if (c < pc[p].nvalJ && (R / 6) <= (Cc / 6)) atomicAdd(C + size_t(Cc) * n + R, -acc[p * 24 + 2 * (ti * 6 + tj) + e]);
+            }
+          }
+        }
+    }
+  }
+}
+
+// One (tile, voxel groups [g_begin, g_end)) work item of the cp.async form: XT staged with 16-B cp.async (zero-fill past a part's
+// columns), SY_STAGES stages of one voxel group each, one CTA barrier per stage, RED epilogue.  k_syrk runs one per CTA, k_syrk_sk a run.
+__device__ __forceinline__ void sy_tile_cp_async(const double* __restrict__ XT, double* __restrict__ C, int W, const SyrkGeom& g, int tile,
+                                                 int g_begin, int g_end, double* smem) {
+  int A, B;
+  sy_tile_parts(g, tile, A, B);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n = 6 * W;
   // part geometry: part I = blocks 2A, 2A+1 (contiguous frames), part J = blocks 2B, 2B+1
   const int colI0 = 6 * sy_gstart(g, 2 * A), ncolI = 6 * (sy_glen(g, 2 * A) + sy_glen(g, 2 * A + 1));
   const int colJ0 = 6 * sy_gstart(g, 2 * B), ncolJ = 6 * (sy_glen(g, 2 * B) + sy_glen(g, 2 * B + 1));
-
-  // enumerate the pieces of this tile in a fixed order and keep those with index % 4 == warp (warp-uniform, <= 3)
   SyPiece pc[3];
-  int npc = 0;
-  {
-    int q = 0;
-    for (int u = 0; u < 4; u++) {
-      const int wy = u >> 1, wx = u & 1, ga = 2 * A + wy, gb = 2 * B + wx;
-      if (!(ga < g.ngc && gb < g.ngc && ga <= gb)) continue;
-      const int nvalI = 6 * sy_glen(g, ga), nvalJ = 6 * sy_glen(g, gb);
-      const int ntI = (nvalI + 7) >> 3, ntJ = (nvalJ + 7) >> 3;
-      for (int t0 = 0; t0 < ntI; t0 += 2, q++) {
-        if ((q & 3) != warp || npc >= 3) continue;
-        SyPiece P;
-        P.offI = (wy ? 6 * sy_glen(g, 2 * A) : 0) + 8 * t0;
-        P.offJ = wx ? 6 * sy_glen(g, 2 * B) : 0;
-        P.ntI = min(2, ntI - t0); P.ntJ = ntJ;
-        P.rowbase = 6 * sy_gstart(g, ga) + 8 * t0; P.colbase = 6 * sy_gstart(g, gb);
-        P.nvalI = nvalI - 8 * t0; P.nvalJ = nvalJ;
-        // tiles of a diagonal unit whose rows all belong to later frames than all of their columns hold only pairs with
-        // frame(i) > frame(j): never stored, so never computed (11 of the 36 tiles of a full diagonal unit)
-        P.mask = 0u;
-        for (int ti = 0; ti < P.ntI; ti++)
-          for (int tj = 0; tj < P.ntJ; tj++)
-            if (!(ga == gb && (8 * (t0 + ti)) / 6 > (8 * tj + 7) / 6)) P.mask |= 1u << (ti * 6 + tj);
-        if (npc == 0) pc[0] = P; else if (npc == 1) pc[1] = P; else pc[2] = P;
-        npc++;
-      }
-    }
-  }
+  const int npc = sy_pieces(g, A, B, warp, pc);
 
   double acc[72];
 #pragma unroll
@@ -544,69 +621,26 @@ __global__ void __launch_bounds__(SY_THREADS, 2) k_syrk(const double* __restrict
     if (step + SY_STAGES - 1 < nsteps) issue(step + SY_STAGES - 1);
     cp_async_commit();
     const double* sI = smem + size_t(step % SY_STAGES) * SY_STAGE_DOUBLES + lane;
-    const double* sJ = sI + SY_PART;
-#pragma unroll
-    for (int p = 0; p < 3; p++) {
-      if (p < npc) {
-        const double* pI = sI + size_t(pc[p].offI) * 4;
-        const double* pJ = sJ + size_t(pc[p].offJ) * 4;
-        const bool full = pc[p].mask == 0xFFFu;
-#pragma unroll
-        for (int kc = 0; kc < 3; kc++) {
-          double fa[2], fb[6];
-#pragma unroll
-          for (int t = 0; t < 2; t++) fa[t] = pI[(kc * SY_PCOLS + 8 * t) * 4];
-#pragma unroll
-          for (int t = 0; t < 6; t++) fb[t] = pJ[(kc * SY_PCOLS + 8 * t) * 4];
-          if (full) {
-#pragma unroll
-            for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-              for (int tj = 0; tj < 6; tj++) dmma884(acc[p * 24 + 2 * (ti * 6 + tj)], acc[p * 24 + 2 * (ti * 6 + tj) + 1], fa[ti], fb[tj]);
-          } else {
-#pragma unroll
-            for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-              for (int tj = 0; tj < 6; tj++)
-                if ((pc[p].mask >> (ti * 6 + tj)) & 1u) dmma884(acc[p * 24 + 2 * (ti * 6 + tj)], acc[p * 24 + 2 * (ti * 6 + tj) + 1], fa[ti], fb[tj]);
-          }
-        }
-      }
-    }
+    sy_stage_mma(acc, pc, npc, sI, sI + SY_PART);
   }
   cp_async_wait<0>();
-  // epilogue: lane holds C[8ti + lane/4][8tj + 2(lane%4) + {0,1}] of every tile; H_ij -= x_i x_j^T for frame(i) <= frame(j)
-  const int rl = lane >> 2, cl = 2 * (lane & 3);
-#pragma unroll
-  for (int p = 0; p < 3; p++) {
-    if (p < npc) {
-#pragma unroll
-      for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-        for (int tj = 0; tj < 6; tj++) {
-          const int r = 8 * ti + rl;
-          if (((pc[p].mask >> (ti * 6 + tj)) & 1u) && r < pc[p].nvalI) {
-            const int R = pc[p].rowbase + r;
-#pragma unroll
-            for (int e = 0; e < 2; e++) {
-              const int c = 8 * tj + cl + e;
-              const int Cc = pc[p].colbase + c;
-              if (c < pc[p].nvalJ && (R / 6) <= (Cc / 6)) atomicAdd(C + size_t(Cc) * n + R, -acc[p * 24 + 2 * (ti * 6 + tj) + e]);
-            }
-          }
-        }
-    }
-  }
+  sy_epilogue(acc, pc, npc, lane, C, n);
 }
 
-// mbarrier / bulk-copy form of k_syrk (the default): same tiling, pieces and epilogue, but
+__global__ void __launch_bounds__(SY_THREADS, 2) k_syrk(const double* __restrict__ XT, double* __restrict__ C, int g_first, int ngroups_vox, int W, SyrkGeom g, int groups_per_chunk, int only_tile) {
+  extern __shared__ __align__(16) double smem[];
+  const int tile = only_tile >= 0 ? only_tile : int(blockIdx.x % g.ntiles), chunk = only_tile >= 0 ? int(blockIdx.x) : int(blockIdx.x / g.ntiles);   // only_tile: diagnostic (cost of one tile kind)
+  const int g_begin = g_first + chunk * groups_per_chunk, g_end = min(ngroups_vox, g_begin + groups_per_chunk);   // voxel groups [g_first, ngroups_vox)
+  if (g_begin >= g_end) return;
+  sy_tile_cp_async(XT, C, W, g, tile, g_begin, g_end, smem);
+}
+
+// mbarrier / bulk-copy form of k_syrk (VXS_SYRK_BULK=1): same tiling, pieces and epilogue, but
 //   * XT is staged by 1-D bulk copies (cp.async.bulk, 3 KB runs: one k-chunk of one part is contiguous in XT) that complete on an mbarrier —
-//     no per-thread loader arithmetic, no cp.async groups, no CTA-wide barrier per stage (the old loop spent ~9 LDGSTS + address math per
-//     thread and one __syncthreads per 108 DMMA per warp; ncu: barrier 1.3 + wait 3.6 stall cycles per issue);
+//     no per-thread loader arithmetic, no cp.async groups, no CTA-wide barrier per stage;
 //   * the warps only meet through the stage barriers: a warp waits for full[s], runs its pieces, arrives on empty[s]; the issuing role
 //     rotates over the warps (lane 0 of warp step%4 refills the stage freed one step ago), so no warp is a dedicated producer and the
-//     2 CTAs x 4 warps x 252 registers still fit the register file;
-//   * the operand fragments of the next (piece, k-chunk) are loaded while the 12 DMMA of the current one issue (explicit double buffer);
+//     2 CTAs x 4 warps still fit the register file;
 //   * a diagonal tile stages its part once (parts I and J are the same columns).
 #define SYB_STAGES 5
 __global__ void __launch_bounds__(SY_THREADS, 2) k_syrk_bulk(const double* __restrict__ XT, double* __restrict__ C, int g_first, int ngroups_vox, int W, SyrkGeom g, int groups_per_chunk) {
@@ -614,9 +648,8 @@ __global__ void __launch_bounds__(SY_THREADS, 2) k_syrk_bulk(const double* __res
   __shared__ __align__(8) uint64_t bars[2 * SYB_STAGES];
   uint64_t* full = bars; uint64_t* empty = bars + SYB_STAGES;
   const int tile = int(blockIdx.x % g.ntiles), chunk = int(blockIdx.x / g.ntiles);
-  int A = 0, rem = tile;
-  while (rem >= g.nbp - A) { rem -= g.nbp - A; A++; }
-  const int B = A + rem;
+  int A, B;
+  sy_tile_parts(g, tile, A, B);
   const int g_begin = g_first + chunk * groups_per_chunk, g_end = min(ngroups_vox, g_begin + groups_per_chunk);
   if (g_begin >= g_end) return;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -624,33 +657,8 @@ __global__ void __launch_bounds__(SY_THREADS, 2) k_syrk_bulk(const double* __res
   const bool diag = (A == B);
   const int colI0 = 6 * sy_gstart(g, 2 * A), ncolI = 6 * (sy_glen(g, 2 * A) + sy_glen(g, 2 * A + 1));
   const int colJ0 = 6 * sy_gstart(g, 2 * B), ncolJ = 6 * (sy_glen(g, 2 * B) + sy_glen(g, 2 * B + 1));
-
   SyPiece pc[3];
-  int npc = 0;
-  {
-    int q = 0;
-    for (int u = 0; u < 4; u++) {
-      const int wy = u >> 1, wx = u & 1, ga = 2 * A + wy, gb = 2 * B + wx;
-      if (!(ga < g.ngc && gb < g.ngc && ga <= gb)) continue;
-      const int nvalI = 6 * sy_glen(g, ga), nvalJ = 6 * sy_glen(g, gb);
-      const int ntI = (nvalI + 7) >> 3, ntJ = (nvalJ + 7) >> 3;
-      for (int t0 = 0; t0 < ntI; t0 += 2, q++) {
-        if ((q & 3) != warp || npc >= 3) continue;
-        SyPiece P;
-        P.offI = (wy ? 6 * sy_glen(g, 2 * A) : 0) + 8 * t0;
-        P.offJ = wx ? 6 * sy_glen(g, 2 * B) : 0;
-        P.ntI = min(2, ntI - t0); P.ntJ = ntJ;
-        P.rowbase = 6 * sy_gstart(g, ga) + 8 * t0; P.colbase = 6 * sy_gstart(g, gb);
-        P.nvalI = nvalI - 8 * t0; P.nvalJ = nvalJ;
-        P.mask = 0u;
-        for (int ti = 0; ti < P.ntI; ti++)
-          for (int tj = 0; tj < P.ntJ; tj++)
-            if (!(ga == gb && (8 * (t0 + ti)) / 6 > (8 * tj + 7) / 6)) P.mask |= 1u << (ti * 6 + tj);
-        if (npc == 0) pc[0] = P; else if (npc == 1) pc[1] = P; else pc[2] = P;
-        npc++;
-      }
-    }
-  }
+  const int npc = sy_pieces(g, A, B, warp, pc);
 
   // the bulk copies only ever write the valid columns of a part: clear the stages once so that the tail columns of a short part hold zeros
   for (int i = tid; i < SYB_STAGES * SY_STAGE_DOUBLES / 2; i += SY_THREADS) reinterpret_cast<double2*>(smem)[i] = make_double2(0.0, 0.0);
@@ -689,77 +697,11 @@ __global__ void __launch_bounds__(SY_THREADS, 2) k_syrk_bulk(const double* __res
     mbar_wait(full + s, ((unsigned)(step / SYB_STAGES)) & 1u);
     const double* sI = smem + size_t(s) * SY_STAGE_DOUBLES + lane;
     const double* sJ = diag ? sI : sI + SY_PART;
-    // fragments of (piece 0, chunk 0)
-    double fa[2][2], fb[2][6];
-    if (npc > 0) {
-      const double* pI = sI + size_t(pc[0].offI) * 4; const double* pJ = sJ + size_t(pc[0].offJ) * 4;
-#pragma unroll
-      for (int t = 0; t < 2; t++) fa[0][t] = pI[(8 * t) * 4];
-#pragma unroll
-      for (int t = 0; t < 6; t++) fb[0][t] = pJ[(8 * t) * 4];
-    }
-#pragma unroll
-    for (int p = 0; p < 3; p++) {
-      if (p < npc) {
-        const bool full_piece = pc[p].mask == 0xFFFu;
-#pragma unroll
-        for (int kc = 0; kc < 3; kc++) {
-          constexpr int dummy = 0; (void)dummy;
-          const int cur = (p * 3 + kc) & 1, nxt = cur ^ 1;
-          // prefetch the fragments of the next (piece, chunk)
-          if (kc < 2) {
-            const double* pI = sI + size_t(pc[p].offI) * 4; const double* pJ = sJ + size_t(pc[p].offJ) * 4;
-#pragma unroll
-            for (int t = 0; t < 2; t++) fa[nxt][t] = pI[((kc + 1) * SY_PCOLS + 8 * t) * 4];
-#pragma unroll
-            for (int t = 0; t < 6; t++) fb[nxt][t] = pJ[((kc + 1) * SY_PCOLS + 8 * t) * 4];
-          } else if (p + 1 < 3 && p + 1 < npc) {
-            const double* pI = sI + size_t(pc[(p + 1) % 3].offI) * 4; const double* pJ = sJ + size_t(pc[(p + 1) % 3].offJ) * 4;
-#pragma unroll
-            for (int t = 0; t < 2; t++) fa[nxt][t] = pI[(8 * t) * 4];
-#pragma unroll
-            for (int t = 0; t < 6; t++) fb[nxt][t] = pJ[(8 * t) * 4];
-          }
-          if (full_piece) {
-#pragma unroll
-            for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-              for (int tj = 0; tj < 6; tj++) dmma884(acc[p * 24 + 2 * (ti * 6 + tj)], acc[p * 24 + 2 * (ti * 6 + tj) + 1], fa[cur][ti], fb[cur][tj]);
-          } else {
-#pragma unroll
-            for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-              for (int tj = 0; tj < 6; tj++)
-                if ((pc[p].mask >> (ti * 6 + tj)) & 1u) dmma884(acc[p * 24 + 2 * (ti * 6 + tj)], acc[p * 24 + 2 * (ti * 6 + tj) + 1], fa[cur][ti], fb[cur][tj]);
-          }
-        }
-      }
-    }
+    sy_stage_mma(acc, pc, npc, sI, sJ);
     __syncwarp();
     if (lane == 0) mbar_arrive(empty + s);
   }
-  // epilogue: lane holds C[8ti + lane/4][8tj + 2(lane%4) + {0,1}] of every tile; H_ij -= x_i x_j^T for frame(i) <= frame(j)
-  const int rl = lane >> 2, cl = 2 * (lane & 3);
-#pragma unroll
-  for (int p = 0; p < 3; p++) {
-    if (p < npc) {
-#pragma unroll
-      for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-        for (int tj = 0; tj < 6; tj++) {
-          const int r = 8 * ti + rl;
-          if (((pc[p].mask >> (ti * 6 + tj)) & 1u) && r < pc[p].nvalI) {
-            const int R = pc[p].rowbase + r;
-#pragma unroll
-            for (int e = 0; e < 2; e++) {
-              const int c = 8 * tj + cl + e;
-              const int Cc = pc[p].colbase + c;
-              if (c < pc[p].nvalJ && (R / 6) <= (Cc / 6)) atomicAdd(C + size_t(Cc) * n + R, -acc[p * 24 + 2 * (ti * 6 + tj) + e]);
-            }
-          }
-        }
-    }
-  }
+  sy_epilogue(acc, pc, npc, lane, C, n);
 }
 
 // Stream-K form of the same kernel: ONE wave of CTAs (2 per SM), every CTA owns a contiguous, equal-cost stretch of the flattened
@@ -770,138 +712,10 @@ struct SySeg { int tile, g_begin, g_end; };
 __global__ void __launch_bounds__(SY_THREADS, 2) k_syrk_sk(const double* __restrict__ XT, double* __restrict__ C, int W, SyrkGeom g, const int* __restrict__ seg_ptr, const SySeg* __restrict__ segs) {
   extern __shared__ __align__(16) double smem[];
   for (int si = seg_ptr[blockIdx.x]; si < seg_ptr[blockIdx.x + 1]; si++) {
-  const int tile = segs[si].tile;
-  int A = 0, rem = tile;
-  while (rem >= g.nbp - A) { rem -= g.nbp - A; A++; }
-  const int B = A + rem;
-  const int g_begin = segs[si].g_begin, g_end = segs[si].g_end;
-  if (g_begin >= g_end) continue;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n = 6 * W;
-  // part geometry: part I = blocks 2A, 2A+1 (contiguous frames), part J = blocks 2B, 2B+1
-  const int colI0 = 6 * sy_gstart(g, 2 * A), ncolI = 6 * (sy_glen(g, 2 * A) + sy_glen(g, 2 * A + 1));
-  const int colJ0 = 6 * sy_gstart(g, 2 * B), ncolJ = 6 * (sy_glen(g, 2 * B) + sy_glen(g, 2 * B + 1));
-
-  // enumerate the pieces of this tile in a fixed order and keep those with index % 4 == warp (warp-uniform, <= 3)
-  SyPiece pc[3];
-  int npc = 0;
-  {
-    int q = 0;
-    for (int u = 0; u < 4; u++) {
-      const int wy = u >> 1, wx = u & 1, ga = 2 * A + wy, gb = 2 * B + wx;
-      if (!(ga < g.ngc && gb < g.ngc && ga <= gb)) continue;
-      const int nvalI = 6 * sy_glen(g, ga), nvalJ = 6 * sy_glen(g, gb);
-      const int ntI = (nvalI + 7) >> 3, ntJ = (nvalJ + 7) >> 3;
-      for (int t0 = 0; t0 < ntI; t0 += 2, q++) {
-        if ((q & 3) != warp || npc >= 3) continue;
-        SyPiece P;
-        P.offI = (wy ? 6 * sy_glen(g, 2 * A) : 0) + 8 * t0;
-        P.offJ = wx ? 6 * sy_glen(g, 2 * B) : 0;
-        P.ntI = min(2, ntI - t0); P.ntJ = ntJ;
-        P.rowbase = 6 * sy_gstart(g, ga) + 8 * t0; P.colbase = 6 * sy_gstart(g, gb);
-        P.nvalI = nvalI - 8 * t0; P.nvalJ = nvalJ;
-        // tiles of a diagonal unit whose rows all belong to later frames than all of their columns hold only pairs with
-        // frame(i) > frame(j): never stored, so never computed (11 of the 36 tiles of a full diagonal unit)
-        P.mask = 0u;
-        for (int ti = 0; ti < P.ntI; ti++)
-          for (int tj = 0; tj < P.ntJ; tj++)
-            if (!(ga == gb && (8 * (t0 + ti)) / 6 > (8 * tj + 7) / 6)) P.mask |= 1u << (ti * 6 + tj);
-        if (npc == 0) pc[0] = P; else if (npc == 1) pc[1] = P; else pc[2] = P;
-        npc++;
-      }
-    }
-  }
-
-  double acc[72];
-#pragma unroll
-  for (int i = 0; i < 72; i++) acc[i] = 0.0;
-
-  const int nsteps = g_end - g_begin;                  // one voxel group (4 voxels, 3 k-chunks) per step
-  constexpr int CH_PER_RUN = SY_PCOLS * 2;             // 16-B chunks per (k-chunk, part) run: 96 cols x 32 B
-  constexpr int CH_PER_STAGE = 3 * 2 * CH_PER_RUN;     // 1152
-  constexpr int CH_PER_THREAD = CH_PER_STAGE / SY_THREADS;   // 9
-  // the loader's address arithmetic does not depend on the step: do it once (source offset inside a voxel group, smem offset, predicate)
-  int ld_src[CH_PER_THREAD], ld_dst[CH_PER_THREAD];
-  unsigned ld_ok = 0;
-#pragma unroll
-  for (int j = 0; j < CH_PER_THREAD; j++) {
-    const int ch = tid + j * SY_THREADS;
-    const int run = ch / CH_PER_RUN, off = ch - run * CH_PER_RUN;      // run = part*3 + kchunk
-    const int part = run / 3, kc = run - part * 3;
-    const int col = off >> 1;                                            // column inside the part
-    const bool ok = col < (part ? ncolJ : ncolI);
-    ld_src[j] = (kc * n + (part ? colJ0 : colI0) + (ok ? col : 0)) * 4 + (off & 1) * 2;
-    ld_dst[j] = part * SY_PART + (kc * SY_PCOLS + col) * 4 + (off & 1) * 2;
-    ld_ok |= (ok ? 1u : 0u) << j;
-  }
-  const size_t group_stride = size_t(3) * n * 4;
-  auto issue = [&](int step) {
-    double* sbase = smem + size_t(step % SY_STAGES) * SY_STAGE_DOUBLES;
-    const double* gbase = XT + size_t(g_begin + step) * group_stride;
-#pragma unroll
-    for (int j = 0; j < CH_PER_THREAD; j++) cp_async16_zfill(sbase + ld_dst[j], gbase + ld_src[j], (ld_ok >> j) & 1u);
-  };
-  for (int s = 0; s < SY_STAGES - 1; s++) { if (s < nsteps) issue(s); cp_async_commit(); }
-  for (int step = 0; step < nsteps; step++) {
-    cp_async_wait<SY_STAGES - 2>();
-    __syncthreads();
-    if (step + SY_STAGES - 1 < nsteps) issue(step + SY_STAGES - 1);
-    cp_async_commit();
-    const double* sI = smem + size_t(step % SY_STAGES) * SY_STAGE_DOUBLES + lane;
-    const double* sJ = sI + SY_PART;
-#pragma unroll
-    for (int p = 0; p < 3; p++) {
-      if (p < npc) {
-        const double* pI = sI + size_t(pc[p].offI) * 4;
-        const double* pJ = sJ + size_t(pc[p].offJ) * 4;
-        const bool full = pc[p].mask == 0xFFFu;
-#pragma unroll
-        for (int kc = 0; kc < 3; kc++) {
-          double fa[2], fb[6];
-#pragma unroll
-          for (int t = 0; t < 2; t++) fa[t] = pI[(kc * SY_PCOLS + 8 * t) * 4];
-#pragma unroll
-          for (int t = 0; t < 6; t++) fb[t] = pJ[(kc * SY_PCOLS + 8 * t) * 4];
-          if (full) {
-#pragma unroll
-            for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-              for (int tj = 0; tj < 6; tj++) dmma884(acc[p * 24 + 2 * (ti * 6 + tj)], acc[p * 24 + 2 * (ti * 6 + tj) + 1], fa[ti], fb[tj]);
-          } else {
-#pragma unroll
-            for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-              for (int tj = 0; tj < 6; tj++)
-                if ((pc[p].mask >> (ti * 6 + tj)) & 1u) dmma884(acc[p * 24 + 2 * (ti * 6 + tj)], acc[p * 24 + 2 * (ti * 6 + tj) + 1], fa[ti], fb[tj]);
-          }
-        }
-      }
-    }
-  }
-  cp_async_wait<0>();
-  // epilogue: lane holds C[8ti + lane/4][8tj + 2(lane%4) + {0,1}] of every tile; H_ij -= x_i x_j^T for frame(i) <= frame(j)
-  const int rl = lane >> 2, cl = 2 * (lane & 3);
-#pragma unroll
-  for (int p = 0; p < 3; p++) {
-    if (p < npc) {
-#pragma unroll
-      for (int ti = 0; ti < 2; ti++)
-#pragma unroll
-        for (int tj = 0; tj < 6; tj++) {
-          const int r = 8 * ti + rl;
-          if (((pc[p].mask >> (ti * 6 + tj)) & 1u) && r < pc[p].nvalI) {
-            const int R = pc[p].rowbase + r;
-#pragma unroll
-            for (int e = 0; e < 2; e++) {
-              const int c = 8 * tj + cl + e;
-              const int Cc = pc[p].colbase + c;
-              if (c < pc[p].nvalJ && (R / 6) <= (Cc / 6)) atomicAdd(C + size_t(Cc) * n + R, -acc[p * 24 + 2 * (ti * 6 + tj) + e]);
-            }
-          }
-        }
-    }
-  }
-  __syncthreads();   // the next segment re-fills the stages
+    const int g_begin = segs[si].g_begin, g_end = segs[si].g_end;
+    if (g_begin >= g_end) continue;
+    sy_tile_cp_async(XT, C, W, g, segs[si].tile, g_begin, g_end, smem);
+    __syncthreads();   // the next segment re-fills the stages
   }
 }
 
@@ -981,27 +795,22 @@ __global__ void k_assemble(const double* __restrict__ C, const double* __restric
 // ------------------------------------------------------------------ host drivers
 static inline unsigned nblk(size_t n, unsigned b) { return unsigned((n + b - 1) / b); }
 
-// cost of one voxel group (one pipeline stage) of a tile = the busiest warp's DMMA count (the warps meet at the stage barrier), by the same
-// piece enumeration as the kernel, + a constant for the stage's barrier / loads
+// cost of one voxel group (one pipeline stage) of a tile = the busiest warp's MMA count (the warps meet at the stage barrier): one m16n8k4
+// per k-chunk and tile column whose ti = 0 tile is needed (sy_mma_chunk), over the kernel's own piece enumeration, + a constant for the
+// stage's barrier / loads
 static int sy_tile_cost(const SyrkGeom& g, int tile) {
-  int A = 0, rem = tile;
-  while (rem >= g.nbp - A) { rem -= g.nbp - A; A++; }
-  const int B = A + rem;
-  int cnt[4] = {0, 0, 0, 0}, npc[4] = {0, 0, 0, 0}, q = 0;
-  for (int u = 0; u < 4; u++) {
-    const int wy = u >> 1, wx = u & 1, ga = 2 * A + wy, gb = 2 * B + wx;
-    if (!(ga < g.ngc && gb < g.ngc && ga <= gb)) continue;
-    const int nvalI = 6 * sy_glen(g, ga), nvalJ = 6 * sy_glen(g, gb), ntI = (nvalI + 7) >> 3, ntJ = (nvalJ + 7) >> 3;
-    for (int t0 = 0; t0 < ntI; t0 += 2, q++) {
-      const int w = q & 3;
-      if (npc[w] >= 3) continue;
-      npc[w]++;
-      for (int ti = 0; ti < std::min(2, ntI - t0); ti++)
-        for (int tj = 0; tj < ntJ; tj++)
-          if (!(ga == gb && (8 * (t0 + ti)) / 6 > (8 * tj + 7) / 6)) cnt[w]++;
-    }
+  int A, B;
+  sy_tile_parts(g, tile, A, B);
+  int busiest = 0;
+  for (int w = 0; w < 4; w++) {
+    SyPiece pc[3];
+    const int npc = sy_pieces(g, A, B, w, pc);
+    int cnt = 0;
+    for (int p = 0; p < npc; p++)
+      for (int tj = 0; tj < 6; tj++) cnt += (pc[p].mask >> tj) & 1u;
+    busiest = std::max(busiest, cnt);
   }
-  return 3 * std::max(std::max(cnt[0], cnt[1]), std::max(cnt[2], cnt[3])) + 6;
+  return 3 * busiest + 6;
 }
 // equal-cost contiguous stretches of the (tile, group) work line for `nctas` CTAs; table = seg_ptr[nctas + 1] | segments x 3 ints
 static int sy_plan(vxs_ctx* ctx, vxs_factor* f, int W, const SyrkGeom& g, int g0, int g1, int nctas) {
@@ -1156,7 +965,8 @@ int vxs_eval_hessian_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, i
           // SYRK over the same groups.  Waves: CTA durations differ by 3x between tile kinds (full off-diagonal / diagonal / remainder) and
           // the CTAs are dispatched in order, so the last wave leaves SMs idle for up to one CTA duration; ncu showed 68.6 % DMMA-pipe
           // activity on average against 85.5 % on the busiest SM at 4 waves.  More, shorter CTAs shrink that tail (each pays one pipeline
-          // fill and one 96x96 RED epilogue); measured at the metric shape: 4 waves 0.781 ms, 8: 0.737, 12: 0.736, 16: 0.742, 24: 0.762.
+          // fill and one 96x96 RED epilogue); k_syrk measured at the metric shape (tools/dmma_shapes.py, H100 80GB HBM3, 700 W power limit,
+          // 1980 MHz): 4 waves 0.576 ms, 8: 0.552, 12: 0.557, 16: 0.568, 24: 0.598.
           if (!chunked && ctx->syrk_streamk && ng >= 8 * ctx->sm_count) {
             int rcs = launch_syrk_sk(ctx, f, C, W, g, g0, g1, smem_sy);
             if (rcs) return rcs;
