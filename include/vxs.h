@@ -205,7 +205,7 @@ int vxs_hba_window(vxs_ctx* ctx, const vxs_map_params* coarse, const vxs_map_par
  *   max_points_per_chunk (<= 0: default 96 Mi): bound on the points of the windows processed together (device memory).
  *   poses_out [nwin][win_size][12]: the windows' refined copies of the poses (the keyframes themselves are not moved, as in the reference);
  *   resis [nwin][2]; status [nwin]: 0, VXS_WARN_SINGULAR or VXS_ERR_TOO_FEW_VOXELS (the reference would exit(0), voxel_map.hpp:345-348 — such a
- *   window keeps its poses); is_converge / lm_iters [nwin]; edges: for pair p = (i, j), i < j in lexicographic order, P = win_size (win_size - 1) / 2
+ *   window keeps its poses, reports is_converge = 0 and resis = {residual1 at its poses, 0}, as damping_iter leaves them at that exit); is_converge / lm_iters [nwin]; edges: for pair p = (i, j), i < j in lexicographic order, P = win_size (win_size - 1) / 2
  *   per window: edge_valid [nwin][P], edge_v6 [nwin][P][6], edge_rot [nwin][P][9], edge_tra [nwin][P][3]; hess_out (may be NULL)
  *   [nwin][(6 win_size)^2] column-major raw Hessians.  Every output but poses_out may be NULL.
  * The submap merge of the reference's post-step (:2428-2447) stays a per-window call (vxs_submap_merge). */

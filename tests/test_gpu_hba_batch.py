@@ -7,6 +7,7 @@ import pytest
 import oracle_api as oa
 import scenes
 import voxel_slam_b200 as vx
+from parity_checks import compare_bottom_window
 
 pytestmark = pytest.mark.gpu
 
@@ -40,22 +41,10 @@ def test_bottom_batch_vs_per_window_oracle(ctx, K, ws, step, pts, stride, chunk)
     win_first = np.arange(0, K - ws + 1, step, dtype=np.int32)
     g = ctx.hba_bottom_batch(fine, xyz, off, est, win_first, win_size=ws, thread_num=2, max_points_per_chunk=chunk, want_hess=True)
     assert np.all(g["status"] == 0)
-    P = ws * (ws - 1) // 2
-    pairs = [(i, j) for i in range(ws) for j in range(i + 1, ws)]
     for w, k0 in enumerate(win_first):
         r, e = oracle_window(fine, xyz, off, est, int(k0), ws)
         assert r["outer_iters"] == 1
-        inc = np.max(np.abs(r["poses"] - est[k0:k0 + ws]))
-        assert np.max(np.abs(g["poses"][w] - r["poses"])) < 1e-5 * inc, (w, np.max(np.abs(g["poses"][w] - r["poses"])), inc)
-        assert np.max(np.abs(g["resis"][w] - r["resis_log"][:2]) / r["resis_log"][:2]) < 1e-7
-        assert np.max(np.abs(g["hess"][w] - r["hess"])) < 1e-6 * np.max(np.abs(r["hess"]))
-        # edges: the same pairs in the same order, variances / relative poses
-        valid = g["edge_valid"][w].astype(bool)
-        ij = np.array([pairs[p] for p in range(P) if valid[p]], dtype=np.int32).reshape(-1, 2)
-        assert e["n"] == len(ij) and np.array_equal(ij, e["ij"])
-        if e["n"]:
-            assert np.max(np.abs(g["edge_v6"][w][valid] - e["v6"]) / e["v6"]) < 1e-5
-            assert np.max(np.abs(g["edge_rot"][w][valid] - e["rot"])) < 1e-8 and np.max(np.abs(g["edge_tra"][w][valid] - e["tra"])) < 1e-7
+        compare_bottom_window(g, w, r, e, est[k0:k0 + ws])     # poses, resis, raw Hessian, and the same edges in the same order
     # the windows move towards the truth
     w = 0
     assert np.abs(g["poses"][w][1:, 9:] - tr[win_first[w] + 1:win_first[w] + ws, 9:]).max() < np.abs(est[1:ws, 9:] - tr[1:ws, 9:]).max()

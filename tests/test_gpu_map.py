@@ -11,10 +11,10 @@ import oracle_api as oa
 import scenes
 import synth
 import voxel_slam_b200 as vx
+from parity_checks import compare_factors
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
-ORDER = ["x", "y", "z", "layer", "path"]
 
 
 @pytest.fixture(scope="module")
@@ -38,29 +38,6 @@ def test_voxel_keys_golden_and_oracle(ctx):
         a, ha = ctx.voxel_keys(p, vs)
         b, hb = oa.voxel_keys(p, vs)
         assert np.array_equal(a, b) and np.array_equal(ha, hb)
-
-
-def compare_factors(f_gpu, ids_gpu, of, W):
-    ex = of.export()
-    assert len(ids_gpu) == of.size(), (len(ids_gpu), of.size())
-    pg, po = np.argsort(ids_gpu, order=ORDER), np.argsort(ex["ids"], order=ORDER)
-    assert np.array_equal(ids_gpu[pg], ex["ids"][po])                       # identical voxel set (root cell, layer, octant path)
-    ptr, fr, cl, fx, co = f_gpu.read_structure()
-    eig, s = f_gpu.read_back()
-    dense = np.zeros((len(ids_gpu), W, 10))
-    vox = np.repeat(np.arange(len(ids_gpu)), np.diff(ptr))
-    dense[vox, fr] = cl
-    assert np.all(np.diff(fr)[np.diff(vox) == 0] > 0)                        # frames ascending within a voxel
-    dg, do = dense[pg], ex["clusters10"][po]
-    assert np.array_equal(dg[:, :, 9], do[:, :, 9])                          # bit-exact per-(voxel, frame) point counts
-    assert np.max(np.abs(dg - do) / (np.abs(do) + 1e-6)) < 1e-12
-    assert np.array_equal(s[pg][:, 9], ex["sum10"][po][:, 9])
-    assert np.max(np.abs(s[pg] - ex["sum10"][po]) / (np.abs(ex["sum10"][po]) + 1e-6)) < 1e-12
-    assert np.max(np.abs(fx[pg] - ex["fix10"][po]) / (np.abs(ex["fix10"][po]) + 1e-6)) < 1e-12
-    assert np.all(co == 1.0)
-    lam_g, lam_o = eig[pg][:, :3], ex["eig12"][po][:, :3]
-    assert np.max(np.abs(lam_g - lam_o) / np.max(np.abs(lam_o), axis=1, keepdims=True)) < 1e-7
-    return pg, po
 
 
 @pytest.mark.parametrize("W,pts,L,max_layer,vs", [(4, 6000, 5.0, 2, 1.0), (10, 20000, 12.0, 2, 1.0), (6, 8000, 6.0, 0, 1.0), (5, 8000, 6.0, 3, 2.0), (7, 5000, 5.0, 1, 0.5)])

@@ -174,7 +174,9 @@ __global__ void __launch_bounds__(128) k_bd_solve(BdState S, const double* __res
 __global__ void __launch_bounds__(128) k_bd_accept(BdState S, int nwin, int WB, int max_iter, int thd_num) {
   const int w = blockIdx.x * blockDim.x + threadIdx.x;
   if (w >= nwin || S.done[w]) return;
-  if (S.nvox[w] < thd_num) { S.status[w] = VXS_ERR_TOO_FEW_VOXELS; S.done[w] = 1; return; }     // "Too Less Voxel" exit(0), voxel_map.hpp:345-348
+  if (S.nvox[w] < thd_num) {     // "Too Less Voxel" exit(0), voxel_map.hpp:345-348: damping_iter has recorded r1 and returns false
+    S.resis[2 * w] = S.r1[w]; S.conv[w] = 0; S.status[w] = VXS_ERR_TOO_FEW_VOXELS; S.done[w] = 1; return;
+  }
   const double r1 = S.r1[w], r2 = S.r2[w];
   if (S.iters[w] == 0) S.resis[2 * w] = r1;
   double q = r1 - r2;
@@ -345,7 +347,10 @@ static int hba_bottom_batch_impl(vxs_ctx* ctx, const vxs_map_params* fine, const
     if (edge_tra) VXS_CUDA(ctx, cudaMemcpyAsync(edge_tra + size_t(w0) * npairs * 3, d_tra, size_t(nw) * npairs * 24, cudaMemcpyDeviceToHost, st));
     if (hess_out) VXS_CUDA(ctx, cudaMemcpyAsync(hess_out + size_t(w0) * n * n, S.Hraw, size_t(nw) * n * n * 8, cudaMemcpyDeviceToHost, st));
     VXS_CUDA(ctx, cudaStreamSynchronize(st));
-    if (V == 0 && status) for (int w = 0; w < nw; w++) status[w0 + w] = VXS_ERR_TOO_FEW_VOXELS;
+    if (V == 0) for (int w = 0; w < nw; w++) {     // no LM iteration ran: r1 = 0 (no voxel), damping_iter returns false as above
+      if (status) status[w0 + w] = VXS_ERR_TOO_FEW_VOXELS;
+      if (is_converge) is_converge[w0 + w] = 0;
+    }
     w0 = w1;
   }
   return warn;
