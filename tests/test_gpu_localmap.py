@@ -8,6 +8,7 @@ import pytest
 import oracle_api as oa
 import synth
 import voxel_slam_b200 as vx
+from parity_checks import compare_factor, compare_leaves, pv_records
 
 pytestmark = pytest.mark.gpu
 
@@ -17,52 +18,6 @@ def ctx():
     c = vx.Context(0)
     yield c
     c.close()
-
-
-def pv_records(scan, seed, full=True):
-    rng = np.random.default_rng(seed)
-    if full:
-        A = rng.standard_normal((scan.shape[0], 3, 3)) * 0.01
-        var = A @ np.transpose(A, (0, 2, 1)) + np.eye(3) * 1e-5
-    else:
-        var = np.broadcast_to(np.eye(3) * 1e-4, (scan.shape[0], 3, 3))
-    return np.concatenate([scan, var.reshape(-1, 9)], axis=1)
-
-
-def leaf_key(s):
-    return np.lexsort(np.concatenate([np.round(s["voxel_center"], 9), s["layer"][:, None]], axis=1).T)
-
-
-def compare_leaves(sg, so, tag, tol=1e-10):
-    assert sg["win_count"] == so["win_count"] and np.array_equal(sg["ring"], so["ring"]), tag
-    kg, ko = leaf_key(sg), leaf_key(so)
-    assert len(kg) == len(ko), (tag, len(kg), len(ko))
-    for f in ("voxel_center", "half", "layer", "is_plane", "isexist", "has_sw", "in_slide", "last_num", "n_point_fix"):
-        assert np.array_equal(sg[f][kg], so[f][ko]), (tag, f, int(np.sum(sg[f][kg] != so[f][ko])))
-    assert np.array_equal(sg["opt_state"][kg] >= 0, so["opt_state"][ko] >= 0), tag
-    for f in ("pcr_add", "pcr_fix", "slots"):
-        x, y = sg[f][kg], so[f][ko]
-        assert np.array_equal(x[..., 9], y[..., 9]), (tag, f)                                      # bit-exact point-to-leaf assignment
-        assert np.max(np.abs(x - y) / (np.abs(y) + 1e-6)) < tol, (tag, f)
-
-
-def compare_factor(f_gpu, of, W, tol=1e-10):
-    ex = of.export()
-    ptr, fr, cl, fx, co = f_gpu.read_structure()
-    eig, s = f_gpu.read_back()
-    assert len(s) == of.size()
-    if len(s) == 0:
-        return
-    kg, ko = np.lexsort(np.round(s[:, [8, 7, 6, 9]], 7).T), np.lexsort(np.round(ex["sum10"][:, [8, 7, 6, 9]], 7).T)     # matched by point count + centroid
-    dense = np.zeros((len(s), W, 10))
-    vox = np.repeat(np.arange(len(s)), np.diff(ptr))
-    dense[vox, fr] = cl
-    assert np.array_equal(dense[kg][:, :, 9], ex["clusters10"][ko][:, :, 9])
-    assert np.max(np.abs(dense[kg] - ex["clusters10"][ko]) / (np.abs(ex["clusters10"][ko]) + 1e-6)) < tol
-    assert np.max(np.abs(s[kg] - ex["sum10"][ko]) / (np.abs(ex["sum10"][ko]) + 1e-6)) < tol
-    assert np.max(np.abs(fx[kg] - ex["fix10"][ko]) / (np.abs(ex["fix10"][ko]) + 1e-6)) < tol
-    lg, lo = eig[kg][:, :3], ex["eig12"][ko][:, :3]
-    assert np.max(np.abs(lg - lo) / np.max(np.abs(lo), axis=1, keepdims=True)) < 1e-7
 
 
 def run_sequence(ctx, Wn, L, nscan, pts, max_layer, max_points, ba_iters, full_var, seed):
