@@ -21,8 +21,8 @@ import voxel_slam_b200 as vx
 
 pytestmark = pytest.mark.gpu
 
-VXS_VARS = ("VXS_SYRK_BULK", "VXS_SYRK_STREAMK", "VXS_SYRK_WAVES", "VXS_SYRK_ONLY_TILE", "VXS_RESID_STREAM", "VXS_RESID_TE", "VXS_RESID_STAGES",
-            "VXS_RESID_PER_SM", "VXS_LDLT_LOOKAHEAD_CTA", "VXS_HBA_ROUTE")
+VXS_VARS = ("VXS_SYRK_WAVES", "VXS_RESID_STREAM", "VXS_RESID_TE", "VXS_RESID_STAGES", "VXS_RESID_PER_SM", "VXS_LDLT_LOOKAHEAD_CTA",
+            "VXS_HBA_ROUTE")
 
 # worst observed error / tolerance per comparator family (printed at the end of the module, run with -s to see it)
 WORST = {}
@@ -328,23 +328,31 @@ def test_hessian_no_fix_unit_coe(ctx):
 
 
 # ------------------------------------------------------------------------------------------------ 4. A/B equivalence of the SYRK forms
-FORMS = {"bulk": dict(VXS_SYRK_BULK=1), "streamk": dict(VXS_SYRK_STREAMK=1), "waves1": dict(VXS_SYRK_WAVES=1), "waves3": dict(VXS_SYRK_WAVES=3),
-         "waves24": dict(VXS_SYRK_WAVES=24)}
-AB_SHAPES = ["W37", "W50", "W129", "W50-streamk-size"]
+FORMS = {"waves1": dict(VXS_SYRK_WAVES=1), "waves3": dict(VXS_SYRK_WAVES=3), "waves24": dict(VXS_SYRK_WAVES=24)}
+AB_SHAPES = ["W37", "W50", "W129", "W50-many-groups"]
 
 
 def ab_case(shape):
-    if shape == "W50-streamk-size":
+    if shape == "W50-many-groups":
         return case(50, 32 * sm_count() + 5, "dense", seed=8)
     return case(int(shape[1:]), 150, "dense", seed=7)
+
+
+def syrk_groups_per_cta(W, V, waves):   # vxs_eval.cu launch_syrk, one upload chunk: voxel groups of 4 per k_syrk CTA
+    r0 = W % 8 or 8
+    nbp = ((W - r0) // 8 + 2) // 2
+    ntiles = nbp * (nbp + 1) // 2
+    ng = (V + 3) // 4
+    nchunks = max(1, min(sm_count() * 2 * waves // ntiles, (ng + 7) // 8))
+    return -(-ng // nchunks)
 
 
 @pytest.mark.parametrize("form", list(FORMS))
 @pytest.mark.parametrize("shape", AB_SHAPES)
 def test_syrk_ab_forms(ctx, env_ctx, shape, form):
     c = ab_case(shape)
-    if shape == "W50-streamk-size":
-        assert c["V"] >= 8 * 4 * sm_count()               # k_syrk_sk engages from 8 voxel groups per SM
+    if shape == "W50-many-groups":
+        assert syrk_groups_per_cta(50, c["V"], 1) > 8        # at one wave the CTA target, not the 8-groups-per-chunk floor, sets the chunks
     base, _ = hessian_on_reused_factor(ctx, c)
     got, ran = hessian_on_reused_factor(env_ctx(**FORMS[form]), c)
     check_path(ran, c)

@@ -31,15 +31,12 @@ extern "C" int vxs_ctx_create(int device, vxs_ctx** out) {
   c->flags.reserve(16);
   { const char* e = getenv("VXS_LDLT_LOOKAHEAD_CTA"); c->ldlt_lookahead = (e && e[0] == '0') ? 0 : 1; }
   { const char* e = getenv("VXS_SYRK_WAVES"); c->syrk_waves = e ? std::max(1, atoi(e)) : 8; }
-  { const char* e = getenv("VXS_SYRK_ONLY_TILE"); c->syrk_only_tile = e ? atoi(e) : -1; }
   { const char* e = getenv("VXS_RESID_STREAM"); c->resid_stream = (e && e[0] == '0') ? 0 : 1; }
   { const char* e = getenv("VXS_RESID_TE"); if (e) c->resid_te = atoi(e); }
   { const char* e = getenv("VXS_RESID_STAGES"); if (e) c->resid_stages = atoi(e); }
   { const char* e = getenv("VXS_RESID_PER_SM"); if (e) c->resid_per_sm = atoi(e); }
   cudaDeviceGetAttribute(&c->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
   { const char* e = getenv("VXS_HBA_ROUTE"); c->hba_route = (e && e[0] == '0') ? 0 : 1; }
-  { const char* e = getenv("VXS_SYRK_BULK"); c->syrk_bulk = (e && e[0] == '1') ? 1 : 0; }
-  { const char* e = getenv("VXS_SYRK_STREAMK"); c->syrk_streamk = (e && e[0] == '1') ? 1 : 0; }
   *out = c;
   return VXS_OK;
 }
@@ -247,7 +244,7 @@ static void factor_free_arrays(vxs_factor* f) {
 }
 static void vxs_factor_release_device(vxs_factor* f) {
   factor_free_arrays(f);
-  f->vwin.release(); f->X.release(); f->C.release(); f->gD.release(); f->partial.release(); f->counter.release(); f->cache_copy.release(); f->sk_tab.release(); f->vc.release();
+  f->vwin.release(); f->X.release(); f->C.release(); f->gD.release(); f->partial.release(); f->counter.release(); f->cache_copy.release(); f->vc.release();
   for (int c = 0; c < vxs_factor::UP_MAX; c++) if (f->up_ev[c]) { cudaEventDestroy(f->up_ev[c]); f->up_ev[c] = nullptr; }
   if (f->up_fence) { cudaEventDestroy(f->up_fence); f->up_fence = nullptr; }
   f->up_pending = f->up_n = 0;

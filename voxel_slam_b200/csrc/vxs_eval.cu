@@ -15,9 +15,7 @@
 //   k_assemble      dense n x n system from the block accumulators (+ the CPU-evaluated IMU 30x30 blocks), mirror of the lower triangle.
 #include <algorithm>
 #include <cstdlib>
-#include <vector>
 #include "vxs_factor_view.cuh"
-#include "vxs_pipe.cuh"
 
 // ------------------------------------------------------------------ residual: transform + sum
 template <int G, bool SP>
@@ -454,8 +452,8 @@ __device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, dou
 }
 
 struct SyrkGeom { int r0, ngc, nbp, ntiles; };
-__host__ __device__ inline int sy_gstart(const SyrkGeom& g, int grp) { return grp <= 0 ? 0 : g.r0 + 8 * (grp - 1); }
-__host__ __device__ inline int sy_glen(const SyrkGeom& g, int grp) { return grp < 0 || grp >= g.ngc ? 0 : (grp == 0 ? g.r0 : 8); }
+__device__ inline int sy_gstart(const SyrkGeom& g, int grp) { return grp <= 0 ? 0 : g.r0 + 8 * (grp - 1); }
+__device__ inline int sy_glen(const SyrkGeom& g, int grp) { return grp < 0 || grp >= g.ngc ? 0 : (grp == 0 ? g.r0 : 8); }
 static SyrkGeom sy_geom(int W) {
   SyrkGeom g;
   g.r0 = (W % 8 == 0) ? 8 : (W % 8);
@@ -471,15 +469,14 @@ static SyrkGeom sy_geom(int W) {
 struct SyPiece { int offI, offJ, ntI, ntJ, rowbase, colbase, nvalI, nvalJ; unsigned mask; };   // mask: bit ti*6+tj = tile needed
 
 // tile index -> (row part A, column part B), A <= B
-__host__ __device__ inline void sy_tile_parts(const SyrkGeom& g, int tile, int& A, int& B) {
+__device__ inline void sy_tile_parts(const SyrkGeom& g, int tile, int& A, int& B) {
   int a = 0, rem = tile;
   while (rem >= g.nbp - a) { rem -= g.nbp - a; a++; }
   A = a; B = a + rem;
 }
 
 // The pieces of tile (A, B) that `warp` runs: the tile's pieces in a fixed order, piece q to warp q % 4 (warp-uniform, <= 3 per warp).
-// The stream-K cost model (sy_tile_cost) counts the same enumeration.
-__host__ __device__ inline int sy_pieces(const SyrkGeom& g, int A, int B, int warp, SyPiece (&pc)[3]) {
+__device__ inline int sy_pieces(const SyrkGeom& g, int A, int B, int warp, SyPiece (&pc)[3]) {
   int npc = 0, q = 0;
   for (int u = 0; u < 4; u++) {
     const int wy = u >> 1, wx = u & 1, ga = 2 * A + wy, gb = 2 * B + wx;
@@ -571,10 +568,13 @@ __device__ __forceinline__ void sy_epilogue(const double (&acc)[72], const SyPie
   }
 }
 
-// One (tile, voxel groups [g_begin, g_end)) work item of the cp.async form: XT staged with 16-B cp.async (zero-fill past a part's
-// columns), SY_STAGES stages of one voxel group each, one CTA barrier per stage, RED epilogue.  k_syrk runs one per CTA, k_syrk_sk a run.
-__device__ __forceinline__ void sy_tile_cp_async(const double* __restrict__ XT, double* __restrict__ C, int W, const SyrkGeom& g, int tile,
-                                                 int g_begin, int g_end, double* smem) {
+// One CTA = one (tile, voxel chunk) work item: XT staged with 16-B cp.async (zero-fill past a part's columns), SY_STAGES stages of one
+// voxel group each, one CTA barrier per stage, RED epilogue.
+__global__ void __launch_bounds__(SY_THREADS, 2) k_syrk(const double* __restrict__ XT, double* __restrict__ C, int g_first, int ngroups_vox, int W, SyrkGeom g, int groups_per_chunk) {
+  extern __shared__ __align__(16) double smem[];
+  const int tile = int(blockIdx.x % g.ntiles), chunk = int(blockIdx.x / g.ntiles);
+  const int g_begin = g_first + chunk * groups_per_chunk, g_end = min(ngroups_vox, g_begin + groups_per_chunk);   // voxel groups [g_first, ngroups_vox)
+  if (g_begin >= g_end) return;
   int A, B;
   sy_tile_parts(g, tile, A, B);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -625,98 +625,6 @@ __device__ __forceinline__ void sy_tile_cp_async(const double* __restrict__ XT, 
   }
   cp_async_wait<0>();
   sy_epilogue(acc, pc, npc, lane, C, n);
-}
-
-__global__ void __launch_bounds__(SY_THREADS, 2) k_syrk(const double* __restrict__ XT, double* __restrict__ C, int g_first, int ngroups_vox, int W, SyrkGeom g, int groups_per_chunk, int only_tile) {
-  extern __shared__ __align__(16) double smem[];
-  const int tile = only_tile >= 0 ? only_tile : int(blockIdx.x % g.ntiles), chunk = only_tile >= 0 ? int(blockIdx.x) : int(blockIdx.x / g.ntiles);   // only_tile: diagnostic (cost of one tile kind)
-  const int g_begin = g_first + chunk * groups_per_chunk, g_end = min(ngroups_vox, g_begin + groups_per_chunk);   // voxel groups [g_first, ngroups_vox)
-  if (g_begin >= g_end) return;
-  sy_tile_cp_async(XT, C, W, g, tile, g_begin, g_end, smem);
-}
-
-// mbarrier / bulk-copy form of k_syrk (VXS_SYRK_BULK=1): same tiling, pieces and epilogue, but
-//   * XT is staged by 1-D bulk copies (cp.async.bulk, 3 KB runs: one k-chunk of one part is contiguous in XT) that complete on an mbarrier —
-//     no per-thread loader arithmetic, no cp.async groups, no CTA-wide barrier per stage;
-//   * the warps only meet through the stage barriers: a warp waits for full[s], runs its pieces, arrives on empty[s]; the issuing role
-//     rotates over the warps (lane 0 of warp step%4 refills the stage freed one step ago), so no warp is a dedicated producer and the
-//     2 CTAs x 4 warps still fit the register file;
-//   * a diagonal tile stages its part once (parts I and J are the same columns).
-#define SYB_STAGES 5
-__global__ void __launch_bounds__(SY_THREADS, 2) k_syrk_bulk(const double* __restrict__ XT, double* __restrict__ C, int g_first, int ngroups_vox, int W, SyrkGeom g, int groups_per_chunk) {
-  extern __shared__ __align__(16) double smem[];
-  __shared__ __align__(8) uint64_t bars[2 * SYB_STAGES];
-  uint64_t* full = bars; uint64_t* empty = bars + SYB_STAGES;
-  const int tile = int(blockIdx.x % g.ntiles), chunk = int(blockIdx.x / g.ntiles);
-  int A, B;
-  sy_tile_parts(g, tile, A, B);
-  const int g_begin = g_first + chunk * groups_per_chunk, g_end = min(ngroups_vox, g_begin + groups_per_chunk);
-  if (g_begin >= g_end) return;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n = 6 * W;
-  const bool diag = (A == B);
-  const int colI0 = 6 * sy_gstart(g, 2 * A), ncolI = 6 * (sy_glen(g, 2 * A) + sy_glen(g, 2 * A + 1));
-  const int colJ0 = 6 * sy_gstart(g, 2 * B), ncolJ = 6 * (sy_glen(g, 2 * B) + sy_glen(g, 2 * B + 1));
-  SyPiece pc[3];
-  const int npc = sy_pieces(g, A, B, warp, pc);
-
-  // the bulk copies only ever write the valid columns of a part: clear the stages once so that the tail columns of a short part hold zeros
-  for (int i = tid; i < SYB_STAGES * SY_STAGE_DOUBLES / 2; i += SY_THREADS) reinterpret_cast<double2*>(smem)[i] = make_double2(0.0, 0.0);
-  if (tid == 0) {
-    for (int s = 0; s < SYB_STAGES; s++) { mbar_init(full + s, 1); mbar_init(empty + s, SY_THREADS / 32); }
-    mbar_fence_init();
-  }
-  fence_proxy_async_smem();
-  __syncthreads();
-
-  const int nsteps = g_end - g_begin;                  // one voxel group (4 voxels, 3 k-chunks) per step
-  const size_t group_stride = size_t(3) * n * 4;
-  const unsigned tx_bytes = 3u * unsigned(ncolI + (diag ? 0 : ncolJ)) * 32u;
-  auto issue = [&](int j) {                            // called by ONE lane
-    const int s = j % SYB_STAGES;
-    mbar_wait(empty + s, (((unsigned)(j / SYB_STAGES)) & 1u) ^ 1u);
-    double* sbase = smem + size_t(s) * SY_STAGE_DOUBLES;
-    const double* gbase = XT + size_t(g_begin + j) * group_stride;
-    mbar_arrive_expect_tx(full + s, tx_bytes);
-#pragma unroll
-    for (int kc = 0; kc < 3; kc++) {
-      bulk_g2s(sbase + kc * SY_PCOLS * 4, gbase + (size_t(kc) * n + colI0) * 4, unsigned(ncolI) * 32u, full + s);
-      if (!diag) bulk_g2s(sbase + SY_PART + kc * SY_PCOLS * 4, gbase + (size_t(kc) * n + colJ0) * 4, unsigned(ncolJ) * 32u, full + s);
-    }
-  };
-  if (tid == 0) for (int j = 0; j < SYB_STAGES - 1 && j < nsteps; j++) issue(j);
-
-  double acc[72];
-#pragma unroll
-  for (int i = 0; i < 72; i++) acc[i] = 0.0;
-
-  for (int step = 0; step < nsteps; step++) {
-    const int s = step % SYB_STAGES;
-    // refill the stage that was consumed one step ago (all four warps arrive on its empty barrier when they leave that step)
-    if (warp == (step & 3) && lane == 0 && step + SYB_STAGES - 1 < nsteps) issue(step + SYB_STAGES - 1);
-    mbar_wait(full + s, ((unsigned)(step / SYB_STAGES)) & 1u);
-    const double* sI = smem + size_t(s) * SY_STAGE_DOUBLES + lane;
-    const double* sJ = diag ? sI : sI + SY_PART;
-    sy_stage_mma(acc, pc, npc, sI, sJ);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(empty + s);
-  }
-  sy_epilogue(acc, pc, npc, lane, C, n);
-}
-
-// Stream-K form of the same kernel: ONE wave of CTAs (2 per SM), every CTA owns a contiguous, equal-cost stretch of the flattened
-// (tile, voxel group) work line computed on the host (sy_plan) — so no in-order dispatch tail, no imbalance between the cheap (diagonal /
-// remainder) and the full tiles, and ~1.3 RED epilogues per CTA instead of one per (tile, chunk) CTA (12 waves x 296 CTAs x 9216 fp64 REDs
-// on the same 45 k addresses before).  seg[b] .. seg[b+1] are CTA b's segments: (tile, first group, end group).
-struct SySeg { int tile, g_begin, g_end; };
-__global__ void __launch_bounds__(SY_THREADS, 2) k_syrk_sk(const double* __restrict__ XT, double* __restrict__ C, int W, SyrkGeom g, const int* __restrict__ seg_ptr, const SySeg* __restrict__ segs) {
-  extern __shared__ __align__(16) double smem[];
-  for (int si = seg_ptr[blockIdx.x]; si < seg_ptr[blockIdx.x + 1]; si++) {
-    const int g_begin = segs[si].g_begin, g_end = segs[si].g_end;
-    if (g_begin >= g_end) continue;
-    sy_tile_cp_async(XT, C, W, g, segs[si].tile, g_begin, g_end, smem);
-    __syncthreads();   // the next segment re-fills the stages
-  }
 }
 
 // ------------------------------------------------------------------ dense system assembly
@@ -795,70 +703,22 @@ __global__ void k_assemble(const double* __restrict__ C, const double* __restric
 // ------------------------------------------------------------------ host drivers
 static inline unsigned nblk(size_t n, unsigned b) { return unsigned((n + b - 1) / b); }
 
-// cost of one voxel group (one pipeline stage) of a tile = the busiest warp's MMA count (the warps meet at the stage barrier): one m16n8k4
-// per k-chunk and tile column whose ti = 0 tile is needed (sy_mma_chunk), over the kernel's own piece enumeration, + a constant for the
-// stage's barrier / loads
-static int sy_tile_cost(const SyrkGeom& g, int tile) {
-  int A, B;
-  sy_tile_parts(g, tile, A, B);
-  int busiest = 0;
-  for (int w = 0; w < 4; w++) {
-    SyPiece pc[3];
-    const int npc = sy_pieces(g, A, B, w, pc);
-    int cnt = 0;
-    for (int p = 0; p < npc; p++)
-      for (int tj = 0; tj < 6; tj++) cnt += (pc[p].mask >> tj) & 1u;
-    busiest = std::max(busiest, cnt);
-  }
-  return 3 * busiest + 6;
-}
-// equal-cost contiguous stretches of the (tile, group) work line for `nctas` CTAs; table = seg_ptr[nctas + 1] | segments x 3 ints
-static int sy_plan(vxs_ctx* ctx, vxs_factor* f, int W, const SyrkGeom& g, int g0, int g1, int nctas) {
-  if (f->sk_key[0] == W && f->sk_key[1] == g0 && f->sk_key[2] == g1 && f->sk_key[3] == nctas && f->sk_tab.p) return VXS_OK;
+// k_syrk over voxel groups [g0, g1) as a (tile, voxel chunk) grid; n_up > 1 when the groups are one of the n_up upload chunks of a
+// chunked first build, which share the waves.  Waves: CTA durations differ by 3x between tile kinds (full off-diagonal / diagonal /
+// remainder) and the CTAs are dispatched in order, so the last wave leaves SMs idle for up to one CTA duration; ncu showed 68.6 % DMMA-pipe
+// activity on average against 85.5 % on the busiest SM at 4 waves.  More, shorter CTAs shrink that tail (each pays one pipeline fill and
+// one 96x96 RED epilogue); k_syrk measured at the metric shape (tools/dmma_shapes.py, H100 80GB HBM3, 700 W power limit, 1980 MHz):
+// 4 waves 0.576 ms, 8: 0.552, 12: 0.557, 16: 0.568, 24: 0.598.
+static int launch_syrk(vxs_ctx* ctx, vxs_factor* f, double* C, int W, int g0, int g1, int n_up) {
+  const SyrkGeom g = sy_geom(W);
   const int ng = g1 - g0;
-  std::vector<double> pre(size_t(g.ntiles) + 1, 0.0);
-  std::vector<int> cost(size_t(g.ntiles));
-  for (int t = 0; t < g.ntiles; t++) { cost[size_t(t)] = sy_tile_cost(g, t); pre[size_t(t) + 1] = pre[size_t(t)] + double(cost[size_t(t)]) * ng; }
-  const double T = pre[size_t(g.ntiles)];
-  // boundary b -> (tile, group) position
-  std::vector<int> bt(size_t(nctas) + 1), bg(size_t(nctas) + 1);
-  for (int b = 0; b <= nctas; b++) {
-    const double c = T * double(b) / double(nctas);
-    int t = 0;
-    while (t < g.ntiles - 1 && pre[size_t(t) + 1] <= c) t++;
-    int o = int((c - pre[size_t(t)]) / double(cost[size_t(t)]) + 0.5);
-    o = std::max(0, std::min(ng, o));
-    bt[size_t(b)] = t; bg[size_t(b)] = o;
-  }
-  bt[size_t(nctas)] = g.ntiles - 1; bg[size_t(nctas)] = ng;
-  std::vector<int> tab(size_t(nctas) + 1);
-  std::vector<int> segs;
-  for (int b = 0; b < nctas; b++) {
-    tab[size_t(b)] = int(segs.size() / 3);
-    int t = bt[size_t(b)], o = bg[size_t(b)];
-    const int te = bt[size_t(b) + 1], oe = bg[size_t(b) + 1];
-    while (t < te) { if (o < ng) { segs.push_back(t); segs.push_back(g0 + o); segs.push_back(g0 + ng); } t++; o = 0; }
-    if (o < oe) { segs.push_back(t); segs.push_back(g0 + o); segs.push_back(g0 + oe); }
-  }
-  tab[size_t(nctas)] = int(segs.size() / 3);
-  const size_t nptr = size_t(nctas) + 1;
-  std::vector<int> all(tab);
-  all.insert(all.end(), segs.begin(), segs.end());
-  VXS_CUDA(ctx, f->sk_tab.reserve(all.size() + 3));
-  VXS_CUDA(ctx, cudaMemcpyAsync(f->sk_tab.p, all.data(), all.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-  VXS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // `all` goes out of scope; plans are cached, so this happens once per window shape
-  f->sk_key[0] = W; f->sk_key[1] = g0; f->sk_key[2] = g1; f->sk_key[3] = nctas;
-  (void)nptr;
-  return VXS_OK;
-}
-static int launch_syrk_sk(vxs_ctx* ctx, vxs_factor* f, double* C, int W, const SyrkGeom& g, int g0, int g1, size_t smem_sy) {
-  const int nctas = ctx->sm_count * 2;
-  int rc = sy_plan(ctx, f, W, g, g0, g1, nctas);
-  if (rc) return rc;
-  VXS_CUDA(ctx, cudaFuncSetAttribute(k_syrk_sk, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_sy)));
-  const int* seg_ptr = f->sk_tab.p;
-  const SySeg* segs = reinterpret_cast<const SySeg*>(f->sk_tab.p + nctas + 1);
-  VXS_LAUNCH(ctx, "k_syrk", k_syrk_sk, unsigned(nctas), SY_THREADS, smem_sy, f->X.p, C, W, g, seg_ptr, segs);
+  const size_t smem = size_t(SY_STAGES) * SY_STAGE_DOUBLES * 8;
+  VXS_CUDA(ctx, cudaFuncSetAttribute(k_syrk, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
+  const int target_ctas = std::max(1, ctx->sm_count * 2 * ctx->syrk_waves / n_up);
+  int nchunks = std::max(1, std::min<int>(target_ctas / g.ntiles, (ng + 7) / 8));
+  const int gpc = (ng + nchunks - 1) / nchunks;
+  nchunks = (ng + gpc - 1) / gpc;
+  VXS_LAUNCH(ctx, "k_syrk", k_syrk, unsigned(nchunks * g.ntiles), SY_THREADS, smem, f->X.p, C, g0, g1, W, g, gpc);
   return VXS_OK;
 }
 static int pick_group(const vxs_factor* f) {
@@ -942,10 +802,6 @@ int vxs_eval_hessian_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, i
     if (dense && W <= 128) {
       const int ngv = int((f->V + 3) / 4);
       const size_t smem = (size_t(30) * 128 + size_t(12) * 7 * W + size_t(12) * W) * 8;
-      const SyrkGeom g = sy_geom(W);
-      const int waves = ctx->syrk_waves;
-      const size_t smem_sy = size_t(SY_STAGES) * SY_STAGE_DOUBLES * 8;
-      VXS_CUDA(ctx, cudaFuncSetAttribute(k_syrk, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_sy)));
       int g0 = 0;
       for (int uc = 0; uc < n_up; uc++) {
         const int g1 = chunked ? std::min(f->up_group_end[uc], ngv) : ngv;
@@ -962,63 +818,23 @@ int vxs_eval_hessian_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, i
             VXS_CUDA(ctx, cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
             VXS_LAUNCH(ctx, "k_jac", kp, grids, 128, smem, fv, poses_dev, pstride, f->X.p, gD, g0, g1);
           }
-          // SYRK over the same groups.  Waves: CTA durations differ by 3x between tile kinds (full off-diagonal / diagonal / remainder) and
-          // the CTAs are dispatched in order, so the last wave leaves SMs idle for up to one CTA duration; ncu showed 68.6 % DMMA-pipe
-          // activity on average against 85.5 % on the busiest SM at 4 waves.  More, shorter CTAs shrink that tail (each pays one pipeline
-          // fill and one 96x96 RED epilogue); k_syrk measured at the metric shape (tools/dmma_shapes.py, H100 80GB HBM3, 700 W power limit,
-          // 1980 MHz): 4 waves 0.576 ms, 8: 0.552, 12: 0.557, 16: 0.568, 24: 0.598.
-          if (!chunked && ctx->syrk_streamk && ng >= 8 * ctx->sm_count) {
-            int rcs = launch_syrk_sk(ctx, f, C, W, g, g0, g1, smem_sy);
-            if (rcs) return rcs;
-          } else {
-            const int target_ctas = std::max(1, ctx->sm_count * 2 * waves / n_up);
-            int nchunks = std::max(1, std::min<int>(target_ctas / g.ntiles, (ng + 7) / 8));
-            const int gpc = (ng + nchunks - 1) / nchunks;
-            nchunks = (ng + gpc - 1) / gpc;
-            const int only = ctx->syrk_only_tile;
-            if (ctx->syrk_bulk && only < 0) {
-              const size_t smem_b = size_t(SYB_STAGES) * SY_STAGE_DOUBLES * 8;
-              VXS_CUDA(ctx, cudaFuncSetAttribute(k_syrk_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_b)));
-              VXS_LAUNCH(ctx, "k_syrk", k_syrk_bulk, unsigned(nchunks * g.ntiles), SY_THREADS, smem_b, f->X.p, C, g0, g1, W, g, gpc);
-            } else
-            VXS_LAUNCH(ctx, "k_syrk", k_syrk, unsigned(only >= 0 ? nchunks : nchunks * g.ntiles), SY_THREADS, smem_sy, f->X.p, C, g0, g1, W, g, gpc, only);
-          }
+          int rcs = launch_syrk(ctx, f, C, W, g0, g1, n_up);   // SYRK over the same groups
+          if (rcs) return rcs;
         }
         g0 = g1;
       }
       if (chunked) f->up_pending = 0;
-    } else if (dense) { if (GJ == 64) LAUNCH_JAC(64, true) else if (GJ == 32) LAUNCH_JAC(32, true) else if (GJ == 16) LAUNCH_JAC(16, true) else LAUNCH_JAC(8, true) }
-    else { if (GJ == 64) LAUNCH_JAC(64, false) else if (GJ == 32) LAUNCH_JAC(32, false) else if (GJ == 16) LAUNCH_JAC(16, false) else LAUNCH_JAC(8, false) }
-#undef LAUNCH_JAC
-    if (dense && W <= 128) {
-      // k_syrk already launched with its Jacobian chunk above
     } else if (dense) {
-      const SyrkGeom g = sy_geom(W);
-      const int ngv = int((f->V + 3) / 4);                 // voxel groups of 4 (12 rows of X each)
-      const int waves = ctx->syrk_waves;
-      int target_ctas = ctx->sm_count * 2 * waves;
-      int nchunks = std::max(1, std::min<int>(target_ctas / g.ntiles, (ngv + 7) / 8));
-      int gpc = (ngv + nchunks - 1) / nchunks;
-      nchunks = (ngv + gpc - 1) / gpc;
-      const size_t smem = size_t(SY_STAGES) * SY_STAGE_DOUBLES * 8;
-      if (ctx->syrk_streamk && ngv >= 8 * ctx->sm_count) {
-        int rcs = launch_syrk_sk(ctx, f, C, W, g, 0, ngv, smem);
-        if (rcs) return rcs;
-      } else {
-        if (ctx->syrk_bulk) {
-          const size_t smem_b = size_t(SYB_STAGES) * SY_STAGE_DOUBLES * 8;
-          VXS_CUDA(ctx, cudaFuncSetAttribute(k_syrk_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem_b)));
-          VXS_LAUNCH(ctx, "k_syrk", k_syrk_bulk, unsigned(nchunks * g.ntiles), SY_THREADS, smem_b, f->X.p, C, 0, ngv, W, g, gpc);
-        } else {
-        VXS_CUDA(ctx, cudaFuncSetAttribute(k_syrk, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-        VXS_LAUNCH(ctx, "k_syrk", k_syrk, unsigned(nchunks * g.ntiles), SY_THREADS, smem, f->X.p, C, 0, ngv, W, g, gpc, -1);
-        }
-      }
+      if (GJ == 64) LAUNCH_JAC(64, true) else if (GJ == 32) LAUNCH_JAC(32, true) else if (GJ == 16) LAUNCH_JAC(16, true) else LAUNCH_JAC(8, true)
+      int rcs = launch_syrk(ctx, f, C, W, 0, int((f->V + 3) / 4), 1);   // voxel groups of 4 (12 rows of X each)
+      if (rcs) return rcs;
     } else {
+      if (GJ == 64) LAUNCH_JAC(64, false) else if (GJ == 32) LAUNCH_JAC(32, false) else if (GJ == 16) LAUNCH_JAC(16, false) else LAUNCH_JAC(8, false)
       if (G == 32) { auto kp = k_pairs<32>; VXS_LAUNCH(ctx, "k_pairs", kp, grid, 128, 0, fv, f->X.p, C); }
       else if (G == 16) { auto kp = k_pairs<16>; VXS_LAUNCH(ctx, "k_pairs", kp, grid, 128, 0, fv, f->X.p, C); }
       else { auto kp = k_pairs<8>; VXS_LAUNCH(ctx, "k_pairs", kp, grid, 128, 0, fv, f->X.p, C); }
     }
+#undef LAUNCH_JAC
     { auto kp = k_eig_residual<false>; VXS_LAUNCH(ctx, "k_lambda_sum", kp, blocks_v, 256, 0, fv, f->partial.p, f->counter.p, r1); }
   }
   if (ctx->nranks > 1) return vxs_comm_allreduce(ctx, C, tot);

@@ -75,18 +75,12 @@ struct vxs_ctx {
   int coop = -1;                  // cooperative launch of k_ldlt_all possible on this device (-1 = not probed yet)
   int ldlt_blocks_per_sm = 0;
   int ldlt_lookahead = 1;         // VXS_LDLT_LOOKAHEAD_CTA=0 keeps the look-ahead on CTA 0 (A/B switch)
-  int syrk_waves = 8;             // VXS_SYRK_WAVES
-  int syrk_only_tile = -1;        // VXS_SYRK_ONLY_TILE: diagnostic, run a single tile kind of k_syrk (results are then incomplete)
+  int syrk_waves = 8;             // VXS_SYRK_WAVES: waves of 2 CTAs per SM the k_syrk grid is cut for (a tuning constant, see launch_syrk)
   int resid_stream = 1;           // VXS_RESID_STREAM=0: k_cluster_sum + k_eig_residual instead of the one streaming kernel (A/B switch)
   int resid_te = 256;             // VXS_RESID_TE: entries per tile (= consumer threads per CTA) of k_residual_stream: 512 (1 CTA/SM), 256 (2), 128 (4)
   int resid_stages = 2, resid_per_sm = 3;   // VXS_RESID_STAGES (2..4), VXS_RESID_PER_SM (CTAs per SM the batches are cut for; 0 = by tile size)
   int smem_optin = 0;             // cudaDevAttrMaxSharedMemoryPerBlockOptin
   int hba_route = 1;              // VXS_HBA_ROUTE=0: multi-GPU top level of vxs_hba_pass through the all-gather of the submaps instead of the owner-routed all-to-all
-  int syrk_bulk = 0;              // VXS_SYRK_BULK=1: the bulk-copy / mbarrier form of k_syrk (A/B switch; measured 0.59 vs 0.55 ms for the cp.async form at the metric
-                                  // shape on an H100 80GB HBM3, 700 W power limit)
-  int syrk_streamk = 0;           // VXS_SYRK_STREAMK=1: one-wave stream-K plan instead of the (tile, chunk) grid of k_syrk (A/B switch; measured SLOWER at the metric
-                                  // shape, 0.71 vs 0.55 ms on the same card: tiles of one voxel chunk no longer run together, so every tile re-reads its XT columns
-                                  // from HBM instead of L2)
   // what ctx->Hraw currently holds (vxs_hba_edges refuses anything but a lidar-only 6W system)
   int hraw_n = 0, hraw_S = 0;
   // solver scratch (n = system size)
@@ -129,8 +123,6 @@ struct vxs_factor {
   DevBuf<double> partial;        // block partial sums for the residual
   DevBuf<unsigned int> counter;
   DevBuf<double> vc;             // [8][Vcap] per-voxel constants for k_jac
-  DevBuf<int> sk_tab;            // stream-K plan of k_syrk_sk: seg_ptr[nctas+1] | segments (tile, g_begin, g_end)
-  int sk_key[4] = {-1, -1, -1, -1};   // (W, g0, g1, nctas) the plan was made for
   DevBuf<double> cache_copy;     // [22][Vcap] snapshot of eig | sum
   size_t cache_copy_V = 0;
   // asynchronous chunked upload (vxs_factor_push_voxels_async): the clusters arrive on ctx->copy_stream in up_n chunks of whole voxel
