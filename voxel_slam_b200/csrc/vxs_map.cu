@@ -183,7 +183,9 @@ __global__ void __launch_bounds__(256) k_map_locate(NodeView nv, unsigned int* _
     }
     if (v == MAP_CLAIM) { leaf_out[i] = MAP_RETRY; atomicAdd(count + 7, 1); return; }
     const int r = int(v - 1u);
-    if (nv.rkey[r] == kx && nv.rkey[nv.cap + r] == ky && nv.rkey[2 * nv.cap + r] == kz) { node = r; break; }
+    // the key of a root another block may have published in this launch: read it at L2 (__ldcg).  A plain load can hit an L1 line cached
+    // before the publication (while probing its neighbours), miss the match, and the probe would then insert the same cell a second time.
+    if (__ldcg(nv.rkey + r) == kx && __ldcg(nv.rkey + nv.cap + r) == ky && __ldcg(nv.rkey + 2 * nv.cap + r) == kz) { node = r; break; }
     h = (h + 1u) & tmask;
   }
   atomicOr(nv.flags + node, F_EXIST | F_SLIDE);          // iter->second->isexist = true; feat_tem_map[position] = ...   :1523-1526

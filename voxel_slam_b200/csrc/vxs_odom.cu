@@ -9,6 +9,9 @@
 // scan.  Leaves partition space, so "descend from the root" == "probe the sorted leaf table with the (root cell, layer, octant path)
 // key of every layer"; the octant path follows the reference's comparisons and float quarter lengths exactly (same routine as the map
 // build), so the point -> leaf assignment is bit-exact.
+// What is bit-exact against the reference: var_init's points, the world points, their root cells and leaves, and the per-point match
+// flags (the gate operands are rounded as the reference rounds them, see vxs_odom_math.cuh).  What is held to a tolerance: var_init's
+// and pvec_update's variances, sigma_l, and the HTH / HTz / nnt sums (fp64 atomics in warp-tree order).
 #include <algorithm>
 #include <cmath>
 #include <vector>
@@ -131,10 +134,11 @@ __global__ void __launch_bounds__(256) k_var_init(const float* __restrict__ pts,
   for (int a = 0; a < 3; a++)
 #pragma unroll
     for (int b = 0; b < 3; b++) var[3 * a + b] = d[a] * rv * d[b] + (A1[a] * dir_var * A1[b] + A2[a] * dir_var * A2[b]);
-  // pv.pnt = ext.R * pv.pnt + ext.p;  pv.var = ext.R * pv.var * ext.R^T     (:199-200)
+  // pv.pnt = ext.R * pv.pnt + ext.p;  pv.var = ext.R * pv.var * ext.R^T     (:199-200).  The point without FMA contraction: the map assigns
+  // it to cells and leaves, so it must round as the reference's does; the variance only feeds sigma and is held to a tolerance.
   double* o = pv + 12 * i;
 #pragma unroll
-  for (int a = 0; a < 3; a++) o[a] = ((ext[3 * a] * pb[0] + ext[3 * a + 1] * pb[1]) + ext[3 * a + 2] * pb[2]) + ext[9 + a];
+  for (int a = 0; a < 3; a++) o[a] = od_dot3(ext[3 * a], ext[3 * a + 1], ext[3 * a + 2], pb[0], pb[1], pb[2], ext[9 + a]);
   double t[9];
 #pragma unroll
   for (int a = 0; a < 3; a++)

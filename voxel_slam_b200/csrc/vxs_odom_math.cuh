@@ -1,6 +1,9 @@
 // The per-point part of the EKF update once the leaf of a world point is known (shared by vxs_odom.cu — exported plane table — and
 // vxs_map.cu — the resident map): OctoTree::match's 3-sigma gates in the reference's float arithmetic (voxel_map.hpp:1339-1363) and the
 // HTH / HTz / nnt / match_num contributions of voxelslam.cpp:900-913.
+// Bit-exact against the reference: the gate operands d, n.d and d.d (rounded intrinsics, no FMA), hence the range gate and, but for
+// sigma_l, the 3-sigma gate.  Held to a tolerance: sigma_l (formed from the upper triangle of plane_var, in another order) and the
+// accumulated sums.  sigma_l can only flip a flag where 3 sqrt(sigma_l) lies within its own rounding of float(|n.d|).
 #pragma once
 #define OD_ROW 28   // per plane: centre 3, normal 3, plane_var upper triangle 21, radius 1
 // r: the 28-double plane row; (x, y, z) body point, (wx, wy, wz) world point, p = pointVar record (pnt 3 | var 9), st = R9 p3 rot_var9 tsl_var9.
@@ -9,10 +12,12 @@ __device__ __forceinline__ int od_contribution(const double* r, double x, double
                                                double* acc) {
   const double R[9] = {st[0], st[1], st[2], st[3], st[4], st[5], st[6], st[7], st[8]};
   const double c[3] = {r[0], r[1], r[2]}, nr[3] = {r[3], r[4], r[5]};
-  const double d[3] = {wx - c[0], wy - c[1], wz - c[2]};
-  const double nd = (nr[0] * d[0] + nr[1] * d[1]) + nr[2] * d[2];
+  // the gate operands in the reference's order and without FMA contraction (voxel_map.hpp:1339-1341): a contracted n.d or d.d rounds
+  // differently, and a point within rounding of a gate then flips its flag
+  const double d[3] = {__dsub_rn(wx, c[0]), __dsub_rn(wy, c[1]), __dsub_rn(wz, c[2])};
+  const double nd = __dadd_rn(__dadd_rn(__dmul_rn(nr[0], d[0]), __dmul_rn(nr[1], d[1])), __dmul_rn(nr[2], d[2]));
   const float dis_to_plane = (float)fabs(nd);
-  const float dis_to_center = (float)((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]);
+  const float dis_to_center = (float)__dadd_rn(__dadd_rn(__dmul_rn(d[0], d[0]), __dmul_rn(d[1], d[1])), __dmul_rn(d[2], d[2]));
   const float range_dis = __fsub_rn(dis_to_center, __fmul_rn(dis_to_plane, dis_to_plane));
   if (!(range_dis <= __fmul_rn(9.0f, (float)r[27]))) return 0;
   // sigma_l = J plane_var J^T + n^T var_world n,  J = [d | -n]
