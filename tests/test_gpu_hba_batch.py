@@ -50,6 +50,24 @@ def test_bottom_batch_vs_per_window_oracle(ctx, K, ws, step, pts, stride, chunk)
     assert np.abs(g["poses"][w][1:, 9:] - tr[win_first[w] + 1:win_first[w] + ws, 9:]).max() < np.abs(est[1:ws, 9:] - tr[1:ws, 9:]).max()
 
 
+def test_bottom_batch_residual_with_poses_from_global_memory(ctx):
+    """32 overlapping windows of 8 (W = 256 frames in one chunk), each owning its copy of a 24 m room's cells: enough voxels that the
+    residual kernel's pose table does not fit in shared memory next to its batch accumulators"""
+    from test_gpu_kernel_paths import resid_plan
+    K, ws, nwin = 39, 8, 32
+    tr, est, xyz, off = trajectory(K, 4000, 24.0, 71)
+    fine = vx.MapParams.make(voxel_size=1.0, min_eigen_value=0.0025, max_layer=2)
+    win_first = np.arange(nwin, dtype=np.int32)
+    V = sum(oa.build_gba_factor(fine, xyz[off[k]:off[k + ws]], off[k:k + ws + 1] - off[k], est[k:k + ws], threads=2).size() for k in win_first)
+    assert not resid_plan(V, nwin * ws)[1], V
+    g = ctx.hba_bottom_batch(fine, xyz, off, est, win_first, win_size=ws, thread_num=2, want_hess=True)
+    assert np.all(g["status"] == 0)
+    for w, k0 in enumerate(win_first):
+        r, e = oracle_window(fine, xyz, off, est, int(k0), ws)
+        assert r["outer_iters"] == 1
+        compare_bottom_window(g, w, r, e, est[k0:k0 + ws])
+
+
 def test_bottom_batch_matches_the_single_window_device_path(ctx):
     K, ws = 15, 10
     tr, est, xyz, off = trajectory(K, 3000, 8.0, 91)

@@ -1,7 +1,7 @@
 """Every Hessian, residual and LDL^T kernel path at its dispatch boundaries and in its A/B forms, CUDA vs the CPU oracle.
 
-The host drivers pick kernels by shape (vxs_eval_hessian_dev, vxs_residual_stream_launch, vxs_solve_damped) and the context picks A/B forms
-from VXS_* environment variables at creation.  Each case here names its shape and switch in its id, checks with the kernel timers that the
+The host drivers pick kernels by shape (vxs_eval_hessian_dev, vxs_residual_stream_launch, vxs_solve_damped) and the context picks the SYRK
+and LDL^T A/B forms from VXS_* environment variables at creation.  Each case here names its shape and switch in its id, checks with the kernel timers that the
 intended kernel ran, and compares with the oracle (the as-written restatement of the reference) at the existing parity tolerances.
 
 Factors of an exact shape are cut from one small synthetic window instead of big map builds: its fully observed voxels are replicated over
@@ -21,8 +21,7 @@ import voxel_slam_b200 as vx
 
 pytestmark = pytest.mark.gpu
 
-VXS_VARS = ("VXS_SYRK_WAVES", "VXS_RESID_STREAM", "VXS_RESID_TE", "VXS_RESID_STAGES", "VXS_RESID_PER_SM", "VXS_LDLT_LOOKAHEAD_CTA",
-            "VXS_HBA_ROUTE")
+VXS_VARS = ("VXS_SYRK_WAVES", "VXS_LDLT_LOOKAHEAD_CTA", "VXS_HBA_ROUTE")
 
 # worst observed error / tolerance per comparator family (printed at the end of the module, run with -s to see it)
 WORST = {}
@@ -372,21 +371,86 @@ def test_chunked_first_build_after_async_push(ctx, W):
 
 
 # ------------------------------------------------------------------------------------------------ 5. residual sweep
-RESID_FORMS = {"default": {}, "te128": dict(VXS_RESID_TE=128), "te512": dict(VXS_RESID_TE=512), "stages3": dict(VXS_RESID_STAGES=3),
-               "stages4": dict(VXS_RESID_STAGES=4), "persm1": dict(VXS_RESID_PER_SM=1), "persm4-te128": dict(VXS_RESID_PER_SM=4, VXS_RESID_TE=128),
-               "two-kernel": dict(VXS_RESID_STREAM=0)}
+def resid_plan(V, W):
+    """vxs_resid.cu vxs_residual_stream_launch: (vbcap, SP) — the batch accumulator rows per CTA and whether the [12][W] pose table fits in the
+    per-CTA shared memory of 3 CTAs per SM next to the 2 stages of 256 entries"""
+    import torch
+    G = 3 * sm_count()
+    m = max(1, (V + G * 48) // (G * 96))
+    VB = -(-V // (G * m))
+    while VB > 256:
+        m += 1
+        VB = -(-V // (G * m))
+    vbcap = (max(VB, 1) + 7) & ~7
+    base = 2 * (10 * 258 * 8 + 256 * 4) + vbcap * 80 + (vbcap + 8) * 4 + 256 * 8 + 2 * 2 * 8 + 128
+    budget = torch.cuda.get_device_properties(0).shared_memory_per_block_optin // 3 - 1024
+    return vbcap, base + 12 * W * 8 <= budget
+
+
+@functools.lru_cache(maxsize=None)
+def csr_case(W, V, k, seed):
+    """A residual factor in CSR form (what push_voxels_async takes), for voxel counts whose dense [V][W][10] arrays would not fit in host
+    memory: each voxel is seen by k frames spread over the window, entry (v, j) is the body-frame cluster of base frame j % 8 of a fully
+    observed base voxel, a world-frame fix cluster on every third voxel, random positive coe."""
+    cl0, est = _base()
+    rng = np.random.default_rng(1000003 * seed + 1009 * W + V)
+    fr = np.sort((rng.integers(W, size=V)[:, None] + np.arange(k) * (W // k)) % W, axis=1)
+    src = (np.arange(V) * 37 + seed) % cl0.shape[0]
+    fix10 = np.zeros((V, 10))
+    for v in range(0, V, 3):
+        fix10[v] = oa.cluster_transform(cl0[src[v], 1], est[1])
+    return dict(W=W, V=V, ptr=np.arange(0, V * k + 1, k, dtype=np.int64), fr=fr.ravel().astype(np.int32), ent=cl0[src[:, None], fr % 8].reshape(-1, 10),
+                fix=fix10, coe=rng.uniform(0.5, 2.0, V), poses=window_poses(W, seed))
+
+
+def csr_clusters(c, a, b):
+    """dense [b - a][W][10] clusters of voxels [a, b) of a csr_case"""
+    ptr, lo, hi = c["ptr"], c["ptr"][a], c["ptr"][b]
+    out = np.zeros((b - a, c["W"], 10))
+    out[np.repeat(np.arange(b - a), np.diff(ptr[a:b + 1])), c["fr"][lo:hi]] = c["ent"][lo:hi]
+    return out
+
+
+def band_w196(): return csr_case(196, 144 * 3 * sm_count() - 1, 4, 15)      # vbcap 144: the smallest W whose pose table can miss
+
+
+def band_w256(): return csr_case(256, 80 * 3 * sm_count(), 4, 16)            # vbcap 80
+
+
 RESID_SHAPES = {
-    "W20": lambda: case(20, 300, "dense", seed=10, empty=0),
-    "W136-full": lambda: case(136, 60, "full", seed=11, single=0, empty=0),       # 136 entries per voxel: more than a TE=128 tile
-    "W300-mixed": lambda: case(300, 80, "mixed", seed=12, stride=10, empty=0),    # > 256 entries (> one default tile), SP = false
-    "W520-mixed": lambda: case(520, 40, "mixed", seed=13, stride=7, empty=0),     # > 512: the two-kernel form reads poses from global too
-    "W16-V7": lambda: case(16, 7, "dense", seed=14, empty=0),                     # fewer voxels than CTAs
+    "W20-sp": lambda: case(20, 300, "dense", seed=10, empty=0),
+    "W136-full-sp": lambda: case(136, 60, "full", seed=11, single=0, empty=0),      # 136 entries per voxel: more than a 128-entry tile
+    "W300-mixed-sp": lambda: case(300, 80, "mixed", seed=12, stride=10, empty=0),   # > 256 entries (> one tile), and a 28.8 KB pose table
+    "W520-mixed-gmem": lambda: case(520, 40, "mixed", seed=13, stride=7, empty=0),  # > 256 entries, poses from global memory
+    "W16-V7-sp": lambda: case(16, 7, "dense", seed=14, empty=0),                    # fewer voxels than CTAs
+    "W196-V144G-gmem": band_w196,
+    "W256-V80G-gmem": band_w256,
+    "W256-V300-sp": lambda: csr_case(256, 300, 4, 17),
 }
 
 
 def eval_poses(c):
     W = c["W"]
     return np.stack([synth.perturb_pose(p, 7 * W + j, 1e-3, 5e-3) for j, p in enumerate(c["poses"])])
+
+
+def residual_ref(c, poses, chunk=2048):
+    """the oracle's evaluate_only_residual and the cache (eig, pcr_add) it leaves, voxel slice by voxel slice so that a slice's dense
+    [n][W][10] arrays stay small; the cache the factor is pushed with does not enter the residual"""
+    r, eig, s = 0.0, [], []
+    for a in range(0, c["V"], chunk):
+        b = min(c["V"], a + chunk)
+        if "ptr" in c:
+            dense = csr_clusters(c, a, b)
+        else:
+            dense = c["cl"][a:b]
+        of = oa.OracleFactor.from_dense(c["W"], dense, None if c["fix"] is None else c["fix"][a:b], None if c["coe"] is None else c["coe"][a:b],
+                                        np.zeros((b - a, 12)), np.zeros((b - a, 10)))
+        r += of.residual(poses)
+        ex = of.export()
+        eig.append(ex["eig12"])
+        s.append(ex["sum10"])
+    return r, np.concatenate(eig), np.concatenate(s)
 
 
 def check_eig(e_gpu, e_ref, tol):
@@ -403,39 +467,40 @@ def check_eig(e_gpu, e_ref, tol):
     return worst
 
 
-def check_residual(r_gpu, eig, s, of, poses):
+def check_residual(r_gpu, eig, s, ref):
     """residual to 1e-10, cached sums to 1e-12, eigenvalues to 1e-7 of lambda_max, eigenvectors to 1e-8 (as test_gpu_ba)"""
-    rr = of.residual(poses)
-    ex = of.export()
+    rr, eig_ref, sum_ref = ref
     er = abs(r_gpu - rr) / abs(rr)
     assert er < 1e-10, er
-    es = relinf(s, ex["sum10"])
+    es = relinf(s, sum_ref)
     assert es < 1e-12, es
-    ee = check_eig(eig, ex["eig12"], 1e-7)
+    ee = check_eig(eig, eig_ref, 1e-7)
     note("residual", max(er / 1e-10, es / 1e-12, ee))
 
 
-@pytest.mark.parametrize("form", list(RESID_FORMS))
 @pytest.mark.parametrize("shape", list(RESID_SHAPES))
-def test_residual_forms(env_ctx, shape, form):
+def test_residual_shapes(ctx, shape):
     c = RESID_SHAPES[shape]()
-    cx = env_ctx(**RESID_FORMS[form])
+    assert resid_plan(c["V"], c["W"])[1] == shape.endswith("-sp")
+    if shape == "W196-V144G-gmem":
+        assert resid_plan(c["V"], c["W"])[0] == 144 and resid_plan(c["V"], 195)[1]
+    if shape == "W256-V80G-gmem":
+        assert resid_plan(c["V"], c["W"])[0] == 80
     poses = eval_poses(c)
-    f = vx.Factor(cx, c["W"])
-    push(f, c)
-    cx.timing_reset()
-    r1 = cx.evaluate_residual(f, poses)
-    ran = ran_kernels(cx)
-    e1, s1 = f.read_back()
-    if form == "two-kernel":
-        assert "k_cluster_sum" in ran and "k_residual_stream" not in ran, ran
+    f = vx.Factor(ctx, c["W"])
+    if "ptr" in c:
+        f.push_voxels_async(c["ptr"], c["fr"], c["ent"], np.zeros((c["V"], 12)), np.zeros((c["V"], 10)), fix10=c["fix"], coe=c["coe"])
     else:
-        assert "k_residual_stream" in ran and "k_cluster_sum" not in ran, ran
-    check_residual(r1, e1, s1, oracle_factor(c), poses)
-    if form != "two-kernel":     # the streaming kernel's reduction order depends only on the factor and the launch shape
-        r2 = cx.evaluate_residual(f, poses)
-        e2, s2 = f.read_back()
-        assert r2 == r1 and np.array_equal(e2, e1) and np.array_equal(s2, s1)
+        push(f, c)
+    ctx.timing_reset()
+    r1 = ctx.evaluate_residual(f, poses)
+    assert "k_residual_stream" in ran_kernels(ctx)
+    e1, s1 = f.read_back()
+    check_residual(r1, e1, s1, residual_ref(c, poses))
+    # the streaming kernel's reduction order depends only on the factor and the launch shape
+    r2 = ctx.evaluate_residual(f, poses)
+    e2, s2 = f.read_back()
+    assert r2 == r1 and np.array_equal(e2, e1) and np.array_equal(s2, s1)
     f.close()
 
 
@@ -588,7 +653,7 @@ def test_negative_control_hessian(ctx):
 
 
 def test_negative_control_residual(ctx):
-    c = RESID_SHAPES["W20"]()
+    c = RESID_SHAPES["W20-sp"]()
     poses = eval_poses(c)
     f = vx.Factor(ctx, c["W"])
     push(f, c, drop_one_entry(c))
@@ -596,7 +661,7 @@ def test_negative_control_residual(ctx):
     e, s = f.read_back()
     f.close()
     with pytest.raises(AssertionError):
-        check_residual(r, e, s, oracle_factor(c), poses)
+        check_residual(r, e, s, residual_ref(c, poses))
 
 
 def test_negative_control_ldlt(ctx):

@@ -6,7 +6,7 @@ timeout 300 python bench.py --impl reference --steps 5 --warmup 1 2> gpurun_out/
 timeout 400 python bench.py --steps 20 --warmup 3 2> gpurun_out/rec_ours.err | grep '^{' > gpurun_out/rec_ours.json
 timeout 300 ncu --metrics gpu__time_duration.sum --clock-control none -c 700 --csv --log-file gpurun_out/launches.csv \
     python bench.py --steps 2 --warmup 3 --no-cpu-baseline > gpurun_out/ncu_launch.log 2>&1
-timeout 400 ncu --set full --clock-control none --import-source on -k regex:"k_syrk|k_jac_slab|k_cluster_sum|k_eig_residual|k_ldlt_all|k_ldlt_solve" -c 6 \
+timeout 400 ncu --set full --clock-control none --import-source on -k regex:"k_syrk|k_jac_slab|k_residual_stream|k_ldlt_all|k_ldlt_solve" -c 6 \
     -f -o gpurun_out/prof_r1_ba python bench.py --steps 1 --warmup 3 --no-cpu-baseline > gpurun_out/ncu_full.log 2>&1
 ls -la gpurun_out | tail -12
 python -c "

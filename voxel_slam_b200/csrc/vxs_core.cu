@@ -31,10 +31,6 @@ extern "C" int vxs_ctx_create(int device, vxs_ctx** out) {
   c->flags.reserve(16);
   { const char* e = getenv("VXS_LDLT_LOOKAHEAD_CTA"); c->ldlt_lookahead = (e && e[0] == '0') ? 0 : 1; }
   { const char* e = getenv("VXS_SYRK_WAVES"); c->syrk_waves = e ? std::max(1, atoi(e)) : 8; }
-  { const char* e = getenv("VXS_RESID_STREAM"); c->resid_stream = (e && e[0] == '0') ? 0 : 1; }
-  { const char* e = getenv("VXS_RESID_TE"); if (e) c->resid_te = atoi(e); }
-  { const char* e = getenv("VXS_RESID_STAGES"); if (e) c->resid_stages = atoi(e); }
-  { const char* e = getenv("VXS_RESID_PER_SM"); if (e) c->resid_per_sm = atoi(e); }
   cudaDeviceGetAttribute(&c->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
   { const char* e = getenv("VXS_HBA_ROUTE"); c->hba_route = (e && e[0] == '0') ? 0 : 1; }
   *out = c;

@@ -1,97 +1,18 @@
-// LidarFactor evaluation kernels (sm_90a): evaluate_only_residual and acc_evaluate2 of the reference
-// (voxel_map.hpp:243-279, 132-241), re-designed for the GPU:
+// LidarFactor evaluation (sm_90a): the kernels of acc_evaluate2 (voxel_map.hpp:132-241), re-designed for the GPU, and the host drivers
+// of both evaluations; evaluate_only_residual (voxel_map.hpp:243-279) is the streaming kernel of vxs_resid.cu.
 //
-//   k_cluster_sum   sub-warp group per voxel, lanes over the voxel's CSR entries; coalesced SoA fp64 loads of the clusters,
-//                   pose gather through the read-only path, cluster transform in registers, shuffle reduction of the
-//                   10 sums, one SoA store per voxel.                                      HBM-bound: (k+1)*80 B / voxel
-//   k_eig_residual  thread per voxel: covariance + fp64 Jacobi eigensolve, SoA store of (lambda,U); deterministic
-//                   two-level reduction of sum coe*lambda0 ("last block" pattern).         176 B / voxel
 //   k_jac           group per voxel, lane per entry: g_i, D_i and the three scaled rank-1 rows x^m_i (SURVEY App. A.3),
 //                   rows stored for the SYRK, g/D accumulated with fp64 RED.                 k*80+176 B read, k*144 B written / voxel
 //   k_syrk          H -= X^T X on the fp64 tensor cores (mma.sync.m16n8k4.f64 / DMMA.16x8x4): warp unit = 48x48 output (8x8 frames,
 //                   6x6 tiles of 8x8, one MMA per pair of tile rows, 72 accumulators/lane), CTA = 2x2 units, X staged with cp.async (zero-fill), 3 stages;
 //                   split over voxel chunks, fp64 RED epilogue.  fp64-bound for k >~ 4 (SURVEY §7.3).
+//   k_lambda_sum    thread per voxel: residual of acc_evaluate2 from the cached eigenvalues, deterministic two-level reduction of
+//                   sum coe*lambda0 ("last block" pattern).
 //   k_pairs         sparse windows (k << W, top-level global BA): group per voxel, block pairs straight to RED.
 //   k_assemble      dense n x n system from the block accumulators (+ the CPU-evaluated IMU 30x30 blocks), mirror of the lower triangle.
 #include <algorithm>
 #include <cstdlib>
 #include "vxs_factor_view.cuh"
-
-// ------------------------------------------------------------------ residual: transform + sum
-template <int G, bool SP>
-__global__ void __launch_bounds__(256) k_cluster_sum(FactorView f, const double* __restrict__ poses, int pstride) {
-  extern __shared__ __align__(16) double sp[];
-  if (SP) stage_poses(sp, poses, pstride, f.W);
-  const int lane = threadIdx.x & (G - 1);
-  const int group = (blockIdx.x * blockDim.x + threadIdx.x) / G;
-  const int ngroups = (gridDim.x * blockDim.x) / G;
-  const int iters = (f.V + ngroups - 1) / ngroups;
-  int nbeg = (group + ngroups < f.V) ? __ldg(f.ptr + group + ngroups) : -1;   // first entry of the voxel of the next iteration
-  for (int it = 0; it < iters; it++) {
-    const int v = group + it * ngroups;
-    const bool valid = v < f.V;
-    int beg = 0, end = 0;
-    if (valid) { beg = f.ptr[v]; end = f.ptr[v + 1]; }
-    const int v2 = v + 2 * ngroups;
-    const int n2beg = (v2 < f.V) ? __ldg(f.ptr + v2) : -1;
-    if (nbeg >= 0) {
-#pragma unroll
-      for (int q = 0; q < (G == 32 ? 2 : 1); q++) prefetch_entry(f, nbeg + lane + q * G);   // a sliding-window voxel has ~W entries
-    }
-    nbeg = n2beg;
-    cluster acc;
-    acc.P.xx = acc.P.xy = acc.P.xz = acc.P.yy = acc.P.yz = acc.P.zz = 0.0; acc.v = mk3(0, 0, 0); acc.n = 0.0;
-    for (int e = beg + lane; e < end; e += G) {
-      cluster c = load_cluster_soa(f.cl, f.Ecap, size_t(e));
-      rot3 R; d3 t;
-      if (SP) load_pose_s(sp, f.W, __ldg(f.frame + e), R, t); else load_pose(poses, pstride, __ldg(f.frame + e), R, t);
-      cluster_transform_acc(c, R, t, acc);
-    }
-    if (G == 32) {
-      // reduce-scatter over the warp: 12 64-bit shuffles instead of 50 (the kernel was LSU-bound on shuffles):
-      // after the five steps the lanes with even index hold one fully reduced component each.
-      double a[10] = {acc.P.xx, acc.P.xy, acc.P.xz, acc.P.yy, acc.P.yz, acc.P.zz, acc.v.x, acc.v.y, acc.v.z, acc.n};
-      const bool b16 = lane & 16, b8 = lane & 8, b4 = lane & 4, b2 = lane & 2;
-      double b[6], c[4], d[2];
-#pragma unroll
-      for (int i = 0; i < 5; i++) { const double keep = b16 ? a[5 + i] : a[i], send = b16 ? a[i] : a[5 + i]; b[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16); }
-      b[5] = 0.0;
-#pragma unroll
-      for (int i = 0; i < 3; i++) { const double keep = b8 ? b[3 + i] : b[i], send = b8 ? b[i] : b[3 + i]; c[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8); }
-      c[3] = 0.0;
-#pragma unroll
-      for (int i = 0; i < 2; i++) { const double keep = b4 ? c[2 + i] : c[i], send = b4 ? c[i] : c[2 + i]; d[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4); }
-      double e = (b2 ? d[1] : d[0]) + __shfl_xor_sync(0xffffffffu, b2 ? d[0] : d[1], 2);
-      e += __shfl_xor_sync(0xffffffffu, e, 1);
-      const int s3 = (b4 ? 2 : 0) + (b2 ? 1 : 0), s2 = b2 ? 1 : 0;
-      const int comp = (b16 ? 5 : 0) + (b8 ? 3 : 0) + s3;
-      const bool holder = !(lane & 1) && s3 < (b8 ? 2 : 3) && s2 < (b4 ? 1 : 2);
-      if (valid && holder) {
-        if (f.has_fix) e += __ldg(f.fix + size_t(comp) * f.Vcap + v);   // PointCluster sig = sig_vecs[a]  (voxel_map.hpp:255)
-        f.sum[size_t(comp) * f.Vcap + v] = e;
-      }
-    } else {
-#pragma unroll
-      for (int off = G / 2; off > 0; off >>= 1) {
-        acc.P.xx += __shfl_xor_sync(0xffffffffu, acc.P.xx, off); acc.P.xy += __shfl_xor_sync(0xffffffffu, acc.P.xy, off);
-        acc.P.xz += __shfl_xor_sync(0xffffffffu, acc.P.xz, off); acc.P.yy += __shfl_xor_sync(0xffffffffu, acc.P.yy, off);
-        acc.P.yz += __shfl_xor_sync(0xffffffffu, acc.P.yz, off); acc.P.zz += __shfl_xor_sync(0xffffffffu, acc.P.zz, off);
-        acc.v.x += __shfl_xor_sync(0xffffffffu, acc.v.x, off); acc.v.y += __shfl_xor_sync(0xffffffffu, acc.v.y, off);
-        acc.v.z += __shfl_xor_sync(0xffffffffu, acc.v.z, off); acc.n += __shfl_xor_sync(0xffffffffu, acc.n, off);
-      }
-      if (valid && lane == 0) {
-        if (f.has_fix) {  // PointCluster sig = sig_vecs[a]  (voxel_map.hpp:255)
-          cluster fx = load_cluster_soa(f.fix, f.Vcap, size_t(v));
-          acc.P.xx += fx.P.xx; acc.P.xy += fx.P.xy; acc.P.xz += fx.P.xz; acc.P.yy += fx.P.yy; acc.P.yz += fx.P.yz; acc.P.zz += fx.P.zz;
-          acc.v = acc.v + fx.v; acc.n += fx.n;
-        }
-        double* s = f.sum + v; const size_t st = f.Vcap;
-        s[0] = acc.P.xx; s[st] = acc.P.xy; s[2 * st] = acc.P.xz; s[3 * st] = acc.P.yy; s[4 * st] = acc.P.yz; s[5 * st] = acc.P.zz;
-        s[6 * st] = acc.v.x; s[7 * st] = acc.v.y; s[8 * st] = acc.v.z; s[9 * st] = acc.n;
-      }
-    }
-  }
-}
 
 // deterministic block + grid reduction of one double per thread; result[0] written by the last block
 __device__ __forceinline__ void block_grid_sum(double val, double* partial, unsigned int* counter, double* result) {
@@ -119,32 +40,10 @@ __device__ __forceinline__ void block_grid_sum(double val, double* partial, unsi
   }
 }
 
-// RECOMPUTE = true : evaluate_only_residual tail (voxel_map.hpp:264-276): cov, eigensolve, cache, r += coe*lambda0
-// RECOMPUTE = false: residual += coe * lmbd[kk] of acc_evaluate2 (voxel_map.hpp:234) from the cached eigenvalues
-template <bool RECOMPUTE>
-__global__ void __launch_bounds__(256) k_eig_residual(FactorView f, double* partial, unsigned int* counter, double* result) {
+// residual += coe * lmbd[kk] of acc_evaluate2 (voxel_map.hpp:234) from the cached eigenvalues
+__global__ void __launch_bounds__(256) k_lambda_sum(FactorView f, double* partial, unsigned int* counter, double* result) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  double contrib = 0.0;
-  if (v < f.V) {
-    const size_t st = f.Vcap;
-    double lam0;
-    if (RECOMPUTE) {
-      cluster s = load_cluster_soa(f.sum, st, size_t(v));
-      sym3 C = cov_from_sum(s);
-      double w[3]; d3 u0, u1, u2;
-      eig3_jacobi(C, w, u0, u1, u2);
-      double* e = f.eig + v;
-      e[0] = w[0]; e[st] = w[1]; e[2 * st] = w[2];
-      e[3 * st] = u0.x; e[4 * st] = u1.x; e[5 * st] = u2.x;
-      e[6 * st] = u0.y; e[7 * st] = u1.y; e[8 * st] = u2.y;
-      e[9 * st] = u0.z; e[10 * st] = u1.z; e[11 * st] = u2.z;
-      lam0 = w[0];
-    } else {
-      lam0 = f.eig[v];
-    }
-    contrib = f.coe[v] * lam0;
-  }
-  block_grid_sum(contrib, partial, counter, result);
+  block_grid_sum(v < f.V ? f.coe[v] * f.eig[v] : 0.0, partial, counter, result);
 }
 
 // per-voxel constants of acc_evaluate2 (voxel_map.hpp:163-174), once per voxel instead of once per (voxel, frame) lane:
@@ -741,28 +640,7 @@ int vxs_eval_residual_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, 
     return VXS_OK;
   }
   { int rcw = vxs_factor_wait_uploads(f); if (rcw) return rcw; }
-  {   // one streaming kernel (vxs_resid.cu); the two-kernel form below is the A/B alternative
-    int ran = 0;
-    int rcs = vxs_residual_stream_launch(ctx, f, poses_dev, pstride, residual_dev, &ran);
-    if (rcs) return rcs;
-    if (ran) { if (ctx->nranks > 1) return vxs_comm_allreduce(ctx, residual_dev, 1); return VXS_OK; }
-  }
-  FactorView fv = make_view(f);
-  const int G = pick_group(f);
-  const unsigned blocks_v = nblk(size_t(f->V), 256);
-  VXS_CUDA(ctx, f->partial.reserve(std::max<size_t>(blocks_v, size_t(ctx->sm_count))));
-  if (!f->counter.p) { VXS_CUDA(ctx, f->counter.reserve(4)); VXS_CUDA(ctx, cudaMemsetAsync(f->counter.p, 0, 16, ctx->stream)); }
-  {
-    const size_t groups_needed = size_t(f->V);
-    unsigned grid = unsigned(std::min<size_t>((groups_needed * G + 255) / 256, size_t(ctx->sm_count) * 8));
-    const bool spm = f->W <= POSE_SMEM_MAX_W;
-    const size_t psm = spm ? size_t(12) * f->W * 8 : 0;
-#define LAUNCH_CS(GG) { if (spm) { auto kp = k_cluster_sum<GG, true>; VXS_LAUNCH(ctx, "k_cluster_sum", kp, grid, 256, psm, fv, poses_dev, pstride); } \
-                        else { auto kp = k_cluster_sum<GG, false>; VXS_LAUNCH(ctx, "k_cluster_sum", kp, grid, 256, 0, fv, poses_dev, pstride); } }
-    if (G == 32) LAUNCH_CS(32) else if (G == 16) LAUNCH_CS(16) else LAUNCH_CS(8)
-#undef LAUNCH_CS
-  }
-  { auto kp = k_eig_residual<true>; VXS_LAUNCH(ctx, "k_eig_residual", kp, blocks_v, 256, 0, fv, f->partial.p, f->counter.p, residual_dev); }
+  { int rcs = vxs_residual_stream_launch(ctx, f, poses_dev, pstride, residual_dev); if (rcs) return rcs; }
   if (ctx->nranks > 1) return vxs_comm_allreduce(ctx, residual_dev, 1);
   return VXS_OK;
 }
@@ -835,7 +713,7 @@ int vxs_eval_hessian_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, i
       else { auto kp = k_pairs<8>; VXS_LAUNCH(ctx, "k_pairs", kp, grid, 128, 0, fv, f->X.p, C); }
     }
 #undef LAUNCH_JAC
-    { auto kp = k_eig_residual<false>; VXS_LAUNCH(ctx, "k_lambda_sum", kp, blocks_v, 256, 0, fv, f->partial.p, f->counter.p, r1); }
+    VXS_LAUNCH(ctx, "k_lambda_sum", k_lambda_sum, blocks_v, 256, 0, fv, f->partial.p, f->counter.p, r1);
   }
   if (ctx->nranks > 1) return vxs_comm_allreduce(ctx, C, tot);
   return VXS_OK;

@@ -38,7 +38,6 @@ __device__ __forceinline__ void load_pose(const double* __restrict__ poses, int 
 
 // Poses staged once per CTA in shared memory, component-major [12][W]: lanes of a group read consecutive frames, so each of the 12
 // reads is one conflict-free wavefront instead of a 96-byte-strided global gather (the LSU, not DRAM, bounds these kernels).
-#define POSE_SMEM_MAX_W 512
 __device__ __forceinline__ void stage_poses(double* sp, const double* __restrict__ poses, int pstride, int W) {
   for (int i = threadIdx.x; i < 12 * W; i += blockDim.x) { const int fr = i / 12, c = i - fr * 12; sp[c * W + fr] = __ldg(poses + size_t(fr) * pstride + c); }
   __syncthreads();

@@ -325,10 +325,8 @@ static int hba_bottom_batch_impl(vxs_ctx* ctx, const vxs_map_params* fine, const
       VXS_LAUNCH(ctx, "k_bd_lambda", k_bd_lambda, unsigned((V + 255) / 256), 256, 0, (const double*)f->eig, (const double*)f->coe, V, B.rvox.p);
       VXS_LAUNCH(ctx, "k_bd_winsum", k_bd_winsum, unsigned(nw), 128, 0, (const double*)B.rvox.p, (const int*)win_ptr, (const unsigned int*)win_vox, (const int*)S.calc, 1, S.r1);
       VXS_LAUNCH(ctx, "k_bd_solve", k_bd_solve, unsigned(nw), 128, smem, S, (const double*)B.Cbd.p, (const double*)B.gD.p, WB, nw);
-      int ran = 0;
-      rc = vxs_residual_stream_launch(ctx, f, S.xt, 12, ctx->scal.p, &ran, B.rvox.p);     // evaluate_only_residual at x_temp: overwrites the cached eig / pcr_adds (:271-273)
+      rc = vxs_residual_stream_launch(ctx, f, S.xt, 12, ctx->scal.p, B.rvox.p);     // evaluate_only_residual at x_temp: overwrites the cached eig / pcr_adds (:271-273)
       if (rc) return rc;
-      if (!ran) return vxs_fail(ctx, VXS_ERR_CUDA, "vxs_hba_bottom_batch: the streaming residual kernel could not be launched");
       VXS_LAUNCH(ctx, "k_bd_winsum", k_bd_winsum, unsigned(nw), 128, 0, (const double*)B.rvox.p, (const int*)win_ptr, (const unsigned int*)win_vox, (const int*)S.done, 0, S.r2);
       VXS_LAUNCH(ctx, "k_bd_accept", k_bd_accept, unsigned((nw + 127) / 128), 128, 0, S, nw, WB, up, thread_num);
     }

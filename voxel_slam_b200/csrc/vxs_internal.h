@@ -76,9 +76,6 @@ struct vxs_ctx {
   int ldlt_blocks_per_sm = 0;
   int ldlt_lookahead = 1;         // VXS_LDLT_LOOKAHEAD_CTA=0 keeps the look-ahead on CTA 0 (A/B switch)
   int syrk_waves = 8;             // VXS_SYRK_WAVES: waves of 2 CTAs per SM the k_syrk grid is cut for (a tuning constant, see launch_syrk)
-  int resid_stream = 1;           // VXS_RESID_STREAM=0: k_cluster_sum + k_eig_residual instead of the one streaming kernel (A/B switch)
-  int resid_te = 256;             // VXS_RESID_TE: entries per tile (= consumer threads per CTA) of k_residual_stream: 512 (1 CTA/SM), 256 (2), 128 (4)
-  int resid_stages = 2, resid_per_sm = 3;   // VXS_RESID_STAGES (2..4), VXS_RESID_PER_SM (CTAs per SM the batches are cut for; 0 = by tile size)
   int smem_optin = 0;             // cudaDevAttrMaxSharedMemoryPerBlockOptin
   int hba_route = 1;              // VXS_HBA_ROUTE=0: multi-GPU top level of vxs_hba_pass through the all-gather of the submaps instead of the owner-routed all-to-all
   // what ctx->Hraw currently holds (vxs_hba_edges refuses anything but a lidar-only 6W system)
@@ -182,7 +179,7 @@ int vxs_eval_residual_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, 
 int vxs_eval_hessian_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, int pose_stride, double* r1_dev);
 int vxs_eval_hessian_bd_dev(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, int pstride, const int* build_mask_dev, double* Cbd, double* gD);
 int vxs_comm_allreduce(vxs_ctx* ctx, double* buf, size_t n);
-int vxs_residual_stream_launch(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, int pstride, double* residual_dev, int* ran, double* rvox = nullptr);   // vxs_resid.cu
+int vxs_residual_stream_launch(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, int pstride, double* residual_dev, double* rvox = nullptr);   // vxs_resid.cu
 
 // solver (vxs_solve.cu)
 int vxs_solve_damped(vxs_ctx* ctx, const double* Hraw, const double* jact, int n, int gauge, double u, double* dx_dev, double* D_dev, double* rhs_dev, int* singular_flag_host);

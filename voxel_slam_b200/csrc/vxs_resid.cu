@@ -1,7 +1,7 @@
 // evaluate_only_residual (voxel_map.hpp:243-279) as ONE streaming kernel (sm_90a):
 //
-//   k_residual_stream   persistent, per_sm CTAs per SM (default: 3 CTAs of TE = 256 consumer threads + one producer warp, 2 stages each; tuned on the
-//                       metric shape, see launch_resid).  The producer warp streams the SoA cluster columns (80 B per (voxel, frame) entry, + the
+//   k_residual_stream   persistent, RS_PER_SM = 3 CTAs per SM of RS_TE = 256 consumer threads + one producer warp, RS_STAGES = 2 stages each
+//                       (tuned on the metric shape, see vxs_residual_stream_launch).  The producer warp streams the SoA cluster columns (80 B per (voxel, frame) entry, + the
 //                       4-B frame index) of the CTA's voxel batches through a ring of shared-memory stages with 1-D bulk copies
 //                       (cp.async.bulk + mbarrier complete_tx — TMA without a tensor map: every column of a tile is one contiguous run),
 //                       so ~130 KB per SM are in flight whatever the consumers do.  TE / 32 consumer warps, per tile of TE entries:
@@ -14,7 +14,7 @@
 //                       Deterministic two-level reduction of the residual ("last block" pattern).
 //
 // Algorithmic bytes (SURVEY.md 8d): (k+1) * 80 B read + 176 B written per voxel; nothing is re-read: the summed cluster never goes
-// back to HBM before the eigensolve (the two-kernel form wrote it and read it again, and paid a second launch).
+// back to HBM before the eigensolve.
 #include <algorithm>
 #include <cstdlib>
 #include "vxs_factor_view.cuh"
@@ -22,31 +22,35 @@
 
 // TE = entries per tile = consumer threads of a CTA (one per entry); + one producer warp.  Smaller CTAs, several per SM, overlap one CTA's
 // reduction / eigensolve phases with another's transform phase (the phases of one CTA run in lock step).
+#define RS_TE 256
+#define RS_PER_SM 3                      // CTAs per SM the batches are cut for and the shared memory is budgeted for
+#define RS_STAGES 2                      // stages of the bulk-copy ring
 #define RS_COLPAD 2                      // doubles of padding between the columns of a stage (bank spread for phase B)
-#define RS_MAX_VB 512                    // voxels per batch (one eigensolve thread each)
-#define RS_MAX_STAGES 4
+#define RS_COL (RS_TE + RS_COLPAD)
+#define RS_STAGE_BYTES (10 * RS_COL * 8 + RS_TE * 4)
 
 struct ResidPlan { int V, VB, nbatch, vbcap; };   // vbcap = VB rounded up to 8: sizes the accumulators / ptr window in shared memory
 
-template <bool SP, int RS_TE>
-__global__ void __launch_bounds__(RS_TE + 32) k_residual_stream(FactorView f, const double* __restrict__ poses, int pstride, ResidPlan pl, int nstages, double* __restrict__ partial,
-                                                                     unsigned int* __restrict__ counter, double* __restrict__ result, double* __restrict__ rvox) {
-  constexpr int RS_CONS = RS_TE, RS_THREADS = RS_TE + 32, RS_COL = RS_TE + RS_COLPAD, RS_STAGE_BYTES = 10 * RS_COL * 8 + RS_TE * 4;
+// SP: the poses are staged in shared memory ([12][W], see load_pose_s) instead of read from global memory; only their source differs
+template <bool SP>
+__global__ void __launch_bounds__(RS_TE + 32) k_residual_stream(FactorView f, const double* __restrict__ poses, int pstride, ResidPlan pl, double* __restrict__ partial,
+                                                                unsigned int* __restrict__ counter, double* __restrict__ result, double* __restrict__ rvox) {
+  constexpr int RS_CONS = RS_TE, RS_THREADS = RS_TE + 32;
   extern __shared__ __align__(128) unsigned char rs_smem[];
   __shared__ int s_va[2], s_vb[2];   // by tile parity: a fast warp writes the next tile's values while a slow one still reads this tile's
   // layout: stages | acc[vbcap][10] | sp_ptr[vbcap + 8] | red[RS_CONS] | barriers | poses [12][W]
   unsigned char* stage_base = rs_smem;
-  double* acc = reinterpret_cast<double*>(rs_smem + size_t(nstages) * RS_STAGE_BYTES);
+  double* acc = reinterpret_cast<double*>(rs_smem + size_t(RS_STAGES) * RS_STAGE_BYTES);
   int* sp_ptr = reinterpret_cast<int*>(acc + pl.vbcap * 10);
   double* red = reinterpret_cast<double*>(sp_ptr + pl.vbcap + 8);
   uint64_t* full = reinterpret_cast<uint64_t*>(red + RS_CONS);
-  uint64_t* empty = full + RS_MAX_STAGES;
-  double* sp = reinterpret_cast<double*>(empty + RS_MAX_STAGES);
+  uint64_t* empty = full + RS_STAGES;
+  double* sp = reinterpret_cast<double*>(empty + RS_STAGES);
   __shared__ bool is_last;
 
   const int tid = threadIdx.x;
   if (tid == 0) {
-    for (int s = 0; s < nstages; s++) { mbar_init(full + s, 1); mbar_init(empty + s, RS_CONS / 32); }
+    for (int s = 0; s < RS_STAGES; s++) { mbar_init(full + s, 1); mbar_init(empty + s, RS_CONS / 32); }
     mbar_fence_init();
   }
   if (SP) { for (int i = tid; i < 12 * f.W; i += RS_THREADS) { const int fr = i / 12, c = i - fr * 12; sp[c * f.W + fr] = __ldg(poses + size_t(fr) * pstride + c); } }
@@ -64,8 +68,8 @@ __global__ void __launch_bounds__(RS_TE + 32) k_residual_stream(FactorView f, co
         const int B0 = __ldg(f.ptr + vb0), B1 = __ldg(f.ptr + vb1);
         const int A0 = B0 & ~3, Bend = (B1 + 3) & ~3;
         for (int t0 = A0; t0 < B1; t0 += RS_TE, tc++) {
-          const int s = int(tc % unsigned(nstages));
-          const unsigned int ph = (tc / unsigned(nstages)) & 1u;
+          const int s = int(tc % unsigned(RS_STAGES));
+          const unsigned int ph = (tc / unsigned(RS_STAGES)) & 1u;
           mbar_wait(empty + s, ph ^ 1u);
           const int cnt = min(RS_TE, Bend - t0);          // multiple of 4 entries: 32-B multiples for the fp64 columns, 16-B for the frames
           unsigned char* st = stage_base + size_t(s) * RS_STAGE_BYTES;
@@ -89,8 +93,8 @@ __global__ void __launch_bounds__(RS_TE + 32) k_residual_stream(FactorView f, co
       const int B0 = sp_ptr[0], B1 = sp_ptr[nv];
       const int A0 = B0 & ~3;
       for (int t0 = A0; t0 < B1; t0 += RS_TE, tc++) {
-        const int s = int(tc % unsigned(nstages));
-        const unsigned int ph = (tc / unsigned(nstages)) & 1u;
+        const int s = int(tc % unsigned(RS_STAGES));
+        const unsigned int ph = (tc / unsigned(RS_STAGES)) & 1u;
         double* col = reinterpret_cast<double*>(stage_base + size_t(s) * RS_STAGE_BYTES);
         const int* frs = reinterpret_cast<const int*>(col + 10 * RS_COL);
         if (lane == 0) mbar_wait(full + s, ph);      // one lane polls (a polling warp costs issue slots the working warps need), the rest of the warp parks at the warp barrier
@@ -191,43 +195,30 @@ __global__ void __launch_bounds__(RS_TE + 32) k_residual_stream(FactorView f, co
   }
 }
 
-// *ran = 1 when the streaming kernel ran, 0 when the caller should use the two-kernel form (A/B switch VXS_RESID_STREAM=0, or no room in shared memory)
-template <bool SP, int TE>
-static int launch_resid(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, int pstride, double* residual_dev, int* ran, double* rvox) {
-  constexpr int COL = TE + RS_COLPAD, STAGE_BYTES = 10 * COL * 8 + TE * 4;
-  // measured at the metric shape (us): TE 512 x 1 CTA/SM x 4 stages 98; 256 x 2 x 4: 81-85; 128 x 4 x 3: 79-81; 256 x 3 x 2: 76 (default); 128 x 6 x 2: 99
-  const int per_sm = TE >= 512 ? 1 : (ctx->resid_per_sm > 0 ? ctx->resid_per_sm : (TE >= 256 ? 2 : 4));
-  const int G = ctx->sm_count * per_sm;
+// Launch shapes tried at the metric shape before the H100 port (us), TE x CTAs/SM x stages: 512 x 1 x 4: 98; 256 x 2 x 4: 81-85; 128 x 4 x 3: 79-81; 256 x 3 x 2: 76 (this one);
+// 128 x 6 x 2: 99.  The bulk copies need 16-B aligned columns: vxs_factor_reserve keeps Ecap a multiple of 32.  Needs f->V > 0.
+int vxs_residual_stream_launch(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, int pstride, double* residual_dev, double* rvox) {
+  const int G = ctx->sm_count * RS_PER_SM;
   // batches: about 96 voxels each, an equal number per CTA
   const long long V = f->V;
   long long m = std::max<long long>(1, (V + (long long)G * 48) / ((long long)G * 96));
   long long VB = (V + (long long)G * m - 1) / ((long long)G * m);
-  while (VB > TE) { m++; VB = (V + (long long)G * m - 1) / ((long long)G * m); }
+  while (VB > RS_TE) { m++; VB = (V + (long long)G * m - 1) / ((long long)G * m); }
   VB = std::max<long long>(VB, 1);
   ResidPlan pl; pl.V = int(V); pl.VB = int(VB); pl.nbatch = int((V + VB - 1) / VB); pl.vbcap = int((VB + 7) & ~7ll);
-  const size_t fixed = size_t(pl.vbcap) * 80 + size_t(pl.vbcap + 8) * 4 + size_t(TE) * 8 + 2 * RS_MAX_STAGES * 8 + (SP ? size_t(12) * f->W * 8 : 0) + 128;
-  const size_t budget = size_t(ctx->smem_optin) / per_sm - (per_sm > 1 ? 1024 : 0);   // per-CTA share (1 KB per CTA is reserved by the driver)
-  int nstages = std::min(RS_MAX_STAGES, std::max(2, ctx->resid_stages));
-  while (nstages > 2 && size_t(nstages) * STAGE_BYTES + fixed > budget) nstages--;
-  if (size_t(nstages) * STAGE_BYTES + fixed > budget) return VXS_OK;
-  const size_t smem = size_t(nstages) * STAGE_BYTES + fixed;
+  const size_t smem_gmem_poses = size_t(RS_STAGES) * RS_STAGE_BYTES + size_t(pl.vbcap) * 80 + size_t(pl.vbcap + 8) * 4 + size_t(RS_TE) * 8 + 2 * RS_STAGES * 8 + 128;
+  const size_t budget = size_t(ctx->smem_optin) / RS_PER_SM - 1024;   // per-CTA share (1 KB per CTA is reserved by the driver)
+  // the pose table goes to shared memory when it fits next to the rest (W <= 195 always does); otherwise the poses are read from global memory,
+  // a plan that needs at most 57 664 B (VB <= 144) of the 76 458 B an H100 CTA gets
+  const bool sp = smem_gmem_poses + size_t(12) * f->W * 8 <= budget;
+  if (!sp && smem_gmem_poses > budget) return vxs_fail(ctx, VXS_ERR_CUDA, "k_residual_stream: not enough shared memory per CTA on this device");
+  const size_t smem = smem_gmem_poses + (sp ? size_t(12) * f->W * 8 : 0);
   const unsigned grid = unsigned(std::min<long long>(G, pl.nbatch));
   VXS_CUDA(ctx, f->partial.reserve(std::max<size_t>(size_t(grid), size_t((V + 255) / 256))));
   if (!f->counter.p) { VXS_CUDA(ctx, f->counter.reserve(4)); VXS_CUDA(ctx, cudaMemsetAsync(f->counter.p, 0, 16, ctx->stream)); }
   FactorView fv = make_view(f);
-  auto kp = k_residual_stream<SP, TE>;
+  auto kp = sp ? k_residual_stream<true> : k_residual_stream<false>;
   VXS_CUDA(ctx, cudaFuncSetAttribute(kp, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)));
-  VXS_LAUNCH(ctx, "k_residual_stream", kp, grid, TE + 32, smem, fv, poses_dev, pstride, pl, nstages, f->partial.p, f->counter.p, residual_dev, rvox);
-  *ran = 1;
+  VXS_LAUNCH(ctx, "k_residual_stream", kp, grid, RS_TE + 32, smem, fv, poses_dev, pstride, pl, f->partial.p, f->counter.p, residual_dev, rvox);
   return VXS_OK;
-}
-int vxs_residual_stream_launch(vxs_ctx* ctx, vxs_factor* f, const double* poses_dev, int pstride, double* residual_dev, int* ran, double* rvox) {
-  *ran = 0;
-  if ((!ctx->resid_stream && !rvox) || f->V <= 0 || (f->Ecap & 3)) return VXS_OK;
-  const bool spm = f->W <= POSE_SMEM_MAX_W && f->W <= 256;
-  const int te = ctx->resid_te;
-#define RS_GO(SPV, TEV) return launch_resid<SPV, TEV>(ctx, f, poses_dev, pstride, residual_dev, ran, rvox)
-  if (spm) { if (te >= 512) RS_GO(true, 512); if (te >= 256) RS_GO(true, 256); RS_GO(true, 128); }
-  if (te >= 512) RS_GO(false, 512); if (te >= 256) RS_GO(false, 256); RS_GO(false, 128);
-#undef RS_GO
 }
