@@ -282,6 +282,10 @@ int vxs_odom_set_planes(vxs_ctx* ctx, const vxs_map_params* mp, int64_t n, const
                         const double* normal, const double* plane_var36, const float* radius);
 int vxs_odom_accumulate(vxs_ctx* ctx, const double* pv12, int64_t n, const double* pose12, const double* rot_var9, const double* tsl_var9,
                         double* HTH36, double* HTz6, double* nnt9, int64_t* match_num, int32_t* flags);
+/* lio_state_estimation (voxelslam.cpp:856-958) in one call against the table of vxs_odom_set_planes; arguments, outputs and errors as
+ * vxs_map_lio_update (below), which shares its driver and its step kernel. */
+int vxs_odom_lio_update(vxs_ctx* ctx, const double* pv12, int64_t n, double* state24, double* cov225, int32_t* ok, int32_t* iters, int64_t* match_num,
+                        double* trace12, int32_t* flags);
 
 /* Point variances of a scan (voxelslam.hpp:187-214; call sites voxelslam.cpp:1246-1250, 1584-1594), the step between down-sampling and the EKF:
  *   vxs_var_init    = var_init: per point calcBodyVar (voxelslam.hpp:163-184: range / bearing noise, dept_err and beam_err narrow to float at the
@@ -322,6 +326,19 @@ int vxs_map_margi(vxs_map* m, const double* poses12, int win_count, int mgsize, 
  * vxs_odom_accumulate; pv12 = NULL uses the ctx's resident scan (vxs_var_init). */
 int vxs_map_odom_accumulate(vxs_map* m, const double* pv12, int64_t n, const double* pose12, const double* rot_var9, const double* tsl_var9, double* HTH36, double* HTz6,
                             double* nnt9, int64_t* match_num, int32_t* flags);
+/* The whole odometry update, lio_state_estimation (voxelslam.cpp:856-958), in one call: cov_inv = cov^-1 once, then up to 4 EKF iterations,
+ * each an association pass (as vxs_map_odom_accumulate, but with the 34 sums reduced in a fixed order, so the result is the same on every run)
+ * followed by the 15x15 update on the device: K_1 = (H_T_H + cov_inv)^-1 (LU with partial pivoting), x_curr += solution (tools.hpp:154-173 Exp /
+ * Log), the convergence test, rematch_num and the stop rule as written; at the stop cov = (I - G) cov and ok = smallest eigenvalue of that
+ * pass's nnt >= 14.  No host round trip between iterations: one read-back and one synchronisation per call.
+ *   pv12 = n pointVar records, NULL = the ctx's resident scan (vxs_var_init / vxs_pvec_update), which must have n records.
+ *   state24 / cov225 (15x15 row-major) in/out: x_curr before and after; g (state24[21..23]) is not touched.
+ *   ok = the reference's return value; iters = iterations executed (2..4); match_num = the last pass's count.
+ *   trace12 (may be NULL): per executed iteration match count, |rot_add|, |tra_add|.  flags (may be NULL): the last pass's per-point match flags.
+ * n == 0 or an empty map: K_1 = cov, G = 0, iters == 2, ok == 0, state and cov unchanged (as the reference).  A cov (or H_T_H + cov_inv) that
+ * meets an exact zero pivot: VXS_ERR_ARG, state24 / cov225 unchanged.  The IMU propagation and the degeneracy counter stay with the caller. */
+int vxs_map_lio_update(vxs_map* m, const double* pv12, int64_t n, double* state24, double* cov225, int32_t* ok, int32_t* iters, int64_t* match_num,
+                       double* trace12, int32_t* flags);
 /* bookkeeping: nodes in the table, points in the point_fix pool, resident scans, ring[win_size] = slot of every logical window position */
 int vxs_map_counts(const vxs_map* m, int64_t* n_nodes, int64_t* n_fix_points, int* win_count, int32_t* ring);
 /* Every leaf of the map, 32 + 10 * win_size doubles each (for tests and debugging): voxel_center 3 | cube half length | layer | is_plane |

@@ -364,9 +364,29 @@ def _pvec_update(self, pv12, pose12, rot_var, tsl_var, n=None, want_pv=True, wan
     return dict(pv=out[:n] if want_pv else None, pwld=pw[:n] if want_pwld else None)
 
 
+def _lio_update(ctx, fn, handle, pv12, state24, cov, n, want_flags):
+    pv = _f64(pv12).reshape(-1, 12) if pv12 is not None else None
+    n = pv.shape[0] if pv is not None else int(n)
+    st, cv = _f64(state24).reshape(24).copy(), _f64(cov).reshape(15, 15).copy()
+    ok, iters, m = C.c_int32(0), C.c_int32(0), C.c_int64(0)
+    trace = np.zeros((4, 3))
+    flags = np.zeros(max(n, 1), dtype=np.int32) if want_flags else None
+    ctx._check(fn(handle, _dp(pv), C.c_int64(n), _dp(st), _dp(cv), C.byref(ok), C.byref(iters), C.byref(m), _dp(trace),
+                  flags.ctypes.data_as(C.POINTER(C.c_int32)) if want_flags else None))
+    return dict(ok=bool(ok.value), state=st, cov=cv, iters=iters.value, n=m.value, trace=trace[: iters.value], flags=flags[:n] if want_flags else None)
+
+
+def _odom_lio_update(self, pv12, state24, cov, n=None, want_flags=False):
+    """lio_state_estimation (voxelslam.cpp:856-958) in one call against the plane table of odom_set_planes: up to 4 EKF iterations on the device.
+    pv12=None = the resident scan (pass n).  Returns ok, state (24), cov (15x15), iters, n (last pass's match count), trace (iters x [match count,
+    |rot_add|, |tra_add|]) and flags (last pass, want_flags)."""
+    return _lio_update(self, lib().vxs_odom_lio_update, self._p, pv12, state24, cov, n, want_flags)
+
+
 Context.var_init = _var_init
 Context.pvec_update = _pvec_update
 Context.odom_set_planes = _odom_set_planes
+Context.odom_lio_update = _odom_lio_update
 Context.odom_accumulate = _odom_accumulate
 
 
@@ -586,6 +606,10 @@ class LocalMap:
         self.ctx._check(lib().vxs_map_odom_accumulate(self._p, _dp(pv), C.c_int64(n), _dp(_f64(pose12)), _dp(_f64(rot_var)), _dp(_f64(tsl_var)), _dp(HTH), _dp(HTz), _dp(nnt), C.byref(m),
                                                       flags.ctypes.data_as(C.POINTER(C.c_int32)) if want_flags else None))
         return dict(n=m.value, HTH=HTH, HTz=HTz, nnt=nnt, flags=flags[:n] if want_flags else None)
+
+    def lio_update(self, pv12, state24, cov, n=None, want_flags=False):
+        """vxs_map_lio_update: lio_state_estimation (voxelslam.cpp:856-958) against the resident map in one call; outputs as Context.odom_lio_update."""
+        return _lio_update(self.ctx, lib().vxs_map_lio_update, self._p, pv12, state24, cov, n, want_flags)
 
     def margi(self, poses12, factor, mgsize=1):
         p = _f64(poses12).reshape(-1, 12)

@@ -446,6 +446,22 @@ inline int odom_accumulate(SurfMap& surf_map, PVecPtr pptr, IMUST& x_curr, bool 
   for (int r = 0; r < 3; r++) for (int c = 0; c < 3; c++) nnt(r, c) = nn[3 * r + c];
   return int(m);
 }
+// lio_state_estimation(pptr) (voxelslam.cpp:856-958, call site :1586) against the resident map in one call: x_curr (R, p, v, bg, ba, cov) is updated
+// in place and the return value is the reference's.  upload = false uses the scan that var_init left on the device (pptr must hold as many points).
+inline bool lio_state_estimation(SurfMap& surf_map, PVecPtr pptr, IMUST& x_curr, bool upload = true) {
+  static_assert(DIM == 15, "cov225 is the 15x15 IMUST::cov");
+  const int64_t n = int64_t(pptr->size());
+  std::vector<double> rec;
+  if (upload) { rec.resize(size_t(n) * 12); for (int64_t i = 0; i < n; i++) { const pointVar& pv = (*pptr)[size_t(i)]; double* q = &rec[12 * size_t(i)]; for (int k = 0; k < 3; k++) q[k] = pv.pnt[k]; for (int r = 0; r < 3; r++) for (int c = 0; c < 3; c++) q[3 + 3 * r + c] = pv.var(r, c); } }
+  double st[24], cov[DIM * DIM];
+  pack_state(x_curr, st);
+  for (int r = 0; r < DIM; r++) for (int c = 0; c < DIM; c++) cov[DIM * r + c] = x_curr.cov(r, c);
+  int32_t ok = 0, iters = 0; int64_t m = 0;
+  check(surf_map.ctx(), vxs_map_lio_update(surf_map.get(), upload ? rec.data() : nullptr, n, st, cov, &ok, &iters, &m, nullptr, nullptr), "vxs_map_lio_update");
+  unpack_state(st, x_curr);
+  for (int r = 0; r < DIM; r++) for (int c = 0; c < DIM; c++) x_curr.cov(r, c) = cov[DIM * r + c];
+  return ok != 0;
+}
 
 // ---------------------------------------------------------------- bottom level of the hierarchical global BA in one call (thd_globalmapping, voxelslam.cpp:2484-2557)
 // every window w solves HBA_add_edge(xs, smp_local, gba_edges1, mps, 1, 2, plptr) on keyframes win_first[w] .. +win_size-1; poses_out[w] are the window's refined xs

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <functional>
 #include <string>
 #include <vector>
 #include "../../include/vxs.h"
@@ -136,6 +137,12 @@ void vxs_hba_release(vxs_ctx* c);
 int vxs_odom_resident_scan(vxs_ctx* ctx, double** pv12_dev, long long* n);            // the scan var_init / odom_accumulate / pvec_update left on the device
 int vxs_odom_set_resident_scan(vxs_ctx* ctx, const double* pv12_host, long long n);
 int vxs_factor_wait_uploads(vxs_factor* f);   // orders ctx->stream behind every pending upload chunk (device-side wait, no host sync)
+// The iterated EKF update of vxs_odom_lio_update / vxs_map_lio_update (vxs_odom.cu): argument checks, the resident scan, the step kernel and the
+// one read-back.  `assoc` enqueues one association pass over the resident scan (pv, n) at the pose in st: `grid` blocks of OD_THREADS points,
+// each writing its partial row of 34 sums to rows, and returning at entry when *stopped is set.  has_map == false: no pass is enqueued.
+typedef std::function<int(unsigned grid, const double* pv, long long n, const double* st, const int* stopped, double* rows, int* flags)> vxs_lio_assoc;
+int vxs_lio_run(vxs_ctx* ctx, const char* who, const double* pv12, int64_t n, bool has_map, const vxs_lio_assoc& assoc, double* state24, double* cov225, int32_t* ok,
+                int32_t* iters, int64_t* match_num, double* trace12, int32_t* flags);
 
 inline int vxs_fail(vxs_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess) {
   if (c) {

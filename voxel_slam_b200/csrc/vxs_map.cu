@@ -688,8 +688,12 @@ __global__ void __launch_bounds__(128) k_map_rehash(NodeView nv, int n_nodes, un
 // match() (voxel_map.hpp:1674-1698): root cell of the world point through the root hash (surf_map holds EVERY root, also those that left the slide
 // map), OctoTree::match (:1335-1392): descend by centre comparison while the node is inner (a missing child ends the search), at the leaf the
 // 3-sigma gates on the plane row that plane_update left in the node — read in place, nothing is exported or re-sorted.
-__global__ void __launch_bounds__(256) k_map_odom(NodeView nv, const unsigned int* __restrict__ table, unsigned int tmask, const double* __restrict__ pv, long long n,
-                                                  const double* __restrict__ st /* R9 p3 rotvar9 tslvar9 */, double voxel_size, double* __restrict__ out, int* __restrict__ flags) {
+// kRows as k_odom_accumulate (vxs_odom.cu): atomic sums for vxs_map_odom_accumulate, partial rows + the stopped flag for vxs_map_lio_update.
+template <bool kRows>
+__global__ void __launch_bounds__(OD_THREADS) k_map_odom(NodeView nv, const unsigned int* __restrict__ table, unsigned int tmask, const double* __restrict__ pv, long long n,
+                                                         const double* __restrict__ st /* R9 p3 rotvar9 tslvar9 */, double voxel_size, double* __restrict__ out, int* __restrict__ flags,
+                                                         const int* __restrict__ stopped) {
+  if (kRows && *stopped) return;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double acc[34];
 #pragma unroll
@@ -718,7 +722,8 @@ __global__ void __launch_bounds__(256) k_map_odom(NodeView nv, const unsigned in
     }
     if (flags) flags[i] = hit;
   }
-  od_flush(acc, out);
+  if (kRows) od_flush_row(acc, out);
+  else od_flush(acc, out);
 }
 
 // ---------------------------------------------------------------- host side
@@ -1198,7 +1203,8 @@ extern "C" int vxs_map_odom_accumulate(vxs_map* m, const double* pv12, int64_t n
   int* dflags = nullptr;
   if (flags && n > 0) { VXS_CUDA(ctx, m->flagbuf.reserve(size_t(n))); dflags = reinterpret_cast<int*>(m->flagbuf.p); }
   if (n > 0 && m->n_nodes > 0)
-    VXS_LAUNCH(ctx, "k_map_odom", k_map_odom, nblk(size_t(n), 256), 256, 0, view(m), m->table.p, (unsigned int)(m->tcap - 1), pv, (long long)n, d_st, m->mp.voxel_size, d_out, dflags);
+    VXS_LAUNCH(ctx, "k_map_odom", k_map_odom<false>, nblk(size_t(n), 256), 256, 0, view(m), m->table.p, (unsigned int)(m->tcap - 1), pv, (long long)n, d_st, m->mp.voxel_size, d_out, dflags,
+               nullptr);
   else if (dflags) VXS_CUDA(ctx, cudaMemsetAsync(dflags, 0, size_t(n) * 4, st));
   double out[34];
   VXS_CUDA(ctx, cudaMemcpyAsync(out, d_out, sizeof out, cudaMemcpyDeviceToHost, st));
@@ -1211,4 +1217,16 @@ extern "C" int vxs_map_odom_accumulate(vxs_map* m, const double* pv12, int64_t n
   for (int k = 0; k < 9; k++) nnt9[k] = out[sy[k]];
   *match_num = int64_t(out[33] + 0.5);
   return VXS_OK;
+}
+
+// lio_state_estimation (voxelslam.cpp:856-958) against the resident map: the driver and the step kernel are vxs_odom.cu's, the passes k_map_odom<true>.
+extern "C" int vxs_map_lio_update(vxs_map* m, const double* pv12, int64_t n, double* state24, double* cov225, int32_t* ok, int32_t* iters, int64_t* match_num, double* trace12,
+                                  int32_t* flags) {
+  if (!m || n < 0 || !state24 || !cov225 || !ok || !iters || !match_num) return VXS_ERR_ARG;
+  vxs_ctx* ctx = m->ctx;
+  auto assoc = [&](unsigned grid, const double* pv, long long np, const double* st, const int* stopped, double* rows, int* fl) -> int {
+    VXS_LAUNCH(ctx, "k_map_odom_rows", k_map_odom<true>, grid, OD_THREADS, 0, view(m), m->table.p, (unsigned int)(m->tcap - 1), pv, np, st, m->mp.voxel_size, rows, fl, stopped);
+    return VXS_OK;
+  };
+  return vxs_lio_run(ctx, "vxs_map_lio_update", pv12, n, m->n_nodes > 0, assoc, state24, cov225, ok, iters, match_num, trace12, flags);
 }

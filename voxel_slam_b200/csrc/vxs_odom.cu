@@ -12,8 +12,11 @@
 // What is bit-exact against the reference: var_init's points, the world points, their root cells and leaves, and the per-point match
 // flags (the gate operands are rounded as the reference rounds them, see vxs_odom_math.cuh).  What is held to a tolerance: var_init's
 // and pvec_update's variances, sigma_l, and the HTH / HTz / nnt sums (fp64 atomics in warp-tree order).
+// The whole iterated update, lio_state_estimation (voxelslam.cpp:856-958), is here too: vxs_lio_run enqueues k_lio_init and 4 x (association
+// pass, k_lio_step) for both association paths (vxs_odom_lio_update, vxs_map_lio_update); its passes sum in a fixed order, not through atomics.
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <vector>
 #include "vxs_internal.h"
 #include "vxs_math.cuh"
@@ -65,6 +68,7 @@ __device__ __forceinline__ unsigned int od_path_prefix(unsigned int bits, int de
 struct OdomScratch {
   DevBuf<unsigned long long> keys;
   DevBuf<double> rows, pts, out, st;
+  DevBuf<double> lio, parts;        // vxs_lio_run: the LioState block and the partial rows of the association passes
   DevBuf<int> flags;
   long long n_planes = 0, n_pts = 0;
   long long minx = 0, miny = 0, minz = 0, ex = 0, ey = 0, ez = 0;
@@ -72,10 +76,14 @@ struct OdomScratch {
   int max_layer = 0;
 };
 
-__global__ void __launch_bounds__(256) k_odom_accumulate(const double* __restrict__ pv, long long n, const double* __restrict__ st /* R9 p3 rotvar9 tslvar9 */,
-                                                         const unsigned long long* __restrict__ keys, const double* __restrict__ rows, long long n_planes, long long minx,
-                                                         long long miny, long long minz, long long ex, long long ey, long long ez, double voxel_size, int max_layer,
-                                                         double* __restrict__ out /* HTH 36 | HTz 6 | nnt 9 | count */, int* __restrict__ flags) {
+// kRows = false: the 34 sums go to `out` through fp64 atomics (vxs_odom_accumulate).  kRows = true (vxs_odom_lio_update): one partial row per
+// block (od_flush_row), and the whole block returns at entry once the EKF step has set *stopped.
+template <bool kRows>
+__global__ void __launch_bounds__(OD_THREADS) k_odom_accumulate(const double* __restrict__ pv, long long n, const double* __restrict__ st /* R9 p3 rotvar9 tslvar9 */,
+                                                                const unsigned long long* __restrict__ keys, const double* __restrict__ rows, long long n_planes, long long minx,
+                                                                long long miny, long long minz, long long ex, long long ey, long long ez, double voxel_size, int max_layer,
+                                                                double* __restrict__ out /* HTH 36 | HTz 6 | nnt 9 | count */, int* __restrict__ flags, const int* __restrict__ stopped) {
+  if (kRows && *stopped) return;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   double acc[34];
 #pragma unroll
@@ -102,7 +110,8 @@ __global__ void __launch_bounds__(256) k_odom_accumulate(const double* __restric
     }
     if (flags) flags[i] = hit;
   }
-  od_flush(acc, out);
+  if (kRows) od_flush_row(acc, out);
+  else od_flush(acc, out);
 }
 
 // calcBodyVar + var_init (voxelslam.hpp:163-203): per point the range / bearing noise model in the sensor frame, then the extrinsic.
@@ -178,6 +187,195 @@ __global__ void __launch_bounds__(256) k_pvec_update(double* __restrict__ pv, lo
   }
 }
 
+// ---------------------------------------------------------------- the iterated EKF update, lio_state_estimation (voxelslam.cpp:856-958)
+// The state of one vxs_*_lio_update call on the device: copied in once and read back once.  The association passes read st and stopped;
+// the step kernel owns the rest.
+struct LioState {
+  double st[30];                 // R9 p3 of x_curr | rot_var9 tsl_var9 = x_curr.cov blocks (0,0), (3,3) (:874-875; fixed until the stop)
+  double x[24], xp[24];          // x_curr, x_prop (state24 layout)
+  double cov[225], cov_inv[225];   // row-major
+  double trace[12];              // per iteration: match_num, |rot_add|, |tra_add|
+  double match_num;              // of the last pass
+  int stopped, iters, rematch, ok, err, pad;
+};
+#define LIO_THREADS 1024
+#define LIO_GROUPS (LIO_THREADS / 34)
+
+// The 15x15 algebra rounds as the reference's scalar code does: products and sums left to right, no FMA contraction.
+__device__ __forceinline__ double lmul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double ladd(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double lsub(double a, double b) { return __dsub_rn(a, b); }
+
+// inv = a^-1 for the row-major 15x15 a (overwritten by its LU factors) as the reference's Matrix<double, 15, 15>::inverse() forms it
+// (PartialPivLU): unblocked right-looking LU, the row pivot the first entry of largest magnitude in the column, the column divided by the
+// pivot, the rank-1 update; then P I solved with the unit-lower and the upper factor, one column per thread.  Returns false to every thread
+// when a pivot is exactly zero (the reference would go on with infinities).
+__device__ bool lio_inverse15(double (*a)[15], double (*inv)[15], int* piv) {
+  const int t = threadIdx.x;
+  for (int k = 0; k < 15; k++) {
+    if (t == 0) {
+      int p = k; double big = fabs(a[k][k]);
+      for (int i = k + 1; i < 15; i++) if (fabs(a[i][k]) > big) { big = fabs(a[i][k]); p = i; }
+      piv[k] = big == 0.0 ? -1 : p;
+    }
+    __syncthreads();
+    const int p = piv[k];
+    if (p < 0) return false;
+    if (p != k && t < 15) { const double v = a[k][t]; a[k][t] = a[p][t]; a[p][t] = v; }
+    __syncthreads();
+    if (t > k && t < 15) a[t][k] = a[t][k] / a[k][k];
+    __syncthreads();
+    const int r = 14 - k;
+    if (t < r * r) { const int i = k + 1 + t / r, j = k + 1 + t % r; a[i][j] = lsub(a[i][j], lmul(a[i][k], a[k][j])); }
+    __syncthreads();
+  }
+  if (t < 15) {
+    for (int i = 0; i < 15; i++) inv[i][t] = i == t ? 1.0 : 0.0;
+    for (int k = 0; k < 15; k++) if (piv[k] != k) { const double v = inv[k][t]; inv[k][t] = inv[piv[k]][t]; inv[piv[k]][t] = v; }
+    for (int j = 0; j < 15; j++) { const double xj = inv[j][t]; for (int i = j + 1; i < 15; i++) inv[i][t] = lsub(inv[i][t], lmul(a[i][j], xj)); }
+    for (int j = 14; j >= 0; j--) { inv[j][t] = inv[j][t] / a[j][j]; const double xj = inv[j][t]; for (int i = 0; i < j; i++) inv[i][t] = lsub(inv[i][t], lmul(a[i][j], xj)); }
+  }
+  __syncthreads();
+  return true;
+}
+
+// cov_inv = x_curr.cov.inverse() (:872), once before the first pass.  A zero pivot stops the update before it starts (err).
+__global__ void __launch_bounds__(LIO_THREADS) k_lio_init(LioState* __restrict__ s) {
+  __shared__ double a[15][15], inv[15][15];
+  __shared__ int piv[15];
+  const int t = threadIdx.x;
+  if (t < 225) a[t / 15][t % 15] = s->cov[t];
+  __syncthreads();
+  if (!lio_inverse15(a, inv, piv)) { if (t == 0) { s->err = 1; s->stopped = 1; } return; }
+  if (t < 225) s->cov_inv[t] = inv[t / 15][t % 15];
+}
+
+// tools.hpp:86-91 Log and 51-66 Exp, in the reference's operation order
+__device__ __forceinline__ void lio_log(const double* R, double* o) {
+  const double tr = ladd(ladd(R[0], R[4]), R[8]);
+  const double th = tr > 3.0 - 1e-6 ? 0.0 : acos(lmul(0.5, lsub(tr, 1.0)));
+  const double K[3] = {lsub(R[7], R[5]), lsub(R[2], R[6]), lsub(R[3], R[1])};
+  const double f = fabs(th) < 0.001 ? 0.5 : lmul(0.5, th) / sin(th);
+  for (int k = 0; k < 3; k++) o[k] = lmul(f, K[k]);
+}
+__device__ __forceinline__ void lio_exp(const double* w, double* E) {
+  const double nn = sqrt(ladd(ladd(lmul(w[0], w[0]), lmul(w[1], w[1])), lmul(w[2], w[2])));
+  for (int k = 0; k < 9; k++) E[k] = (k % 4 == 0) ? 1.0 : 0.0;
+  if (!(nn >= 1e-11)) return;
+  const double r[3] = {w[0] / nn, w[1] / nn, w[2] / nn};
+  const double K[9] = {0.0, -r[2], r[1], r[2], 0.0, -r[0], -r[1], r[0], 0.0};
+  const double s = sin(nn), c = lsub(1.0, cos(nn));
+  double cK[9];
+  for (int k = 0; k < 9; k++) cK[k] = lmul(c, K[k]);
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) {
+      double kk = lmul(cK[3 * i], K[j]);
+      for (int q = 1; q < 3; q++) kk = ladd(kk, lmul(cK[3 * i + q], K[3 * q + j]));
+      E[3 * i + j] = ladd(ladd(E[3 * i + j], lmul(s, K[3 * i + j])), kk);
+    }
+}
+
+// One iteration of the EKF loop (voxelslam.cpp:873-948) against the partial rows of the pass before it; one CTA.  Returns at entry once
+// the update has stopped.  The partial rows are summed in a fixed order, so the iteration is bit-reproducible.
+__global__ void __launch_bounds__(LIO_THREADS) k_lio_step(LioState* __restrict__ s, const double* __restrict__ rows, int nrows) {
+  if (s->stopped) return;
+  __shared__ double red[LIO_GROUPS][34];
+  __shared__ double sum[34], HTH[6][6], a[15][15], K1[15][15], G[15][6], vec[15], sol[15], ncov[225];
+  __shared__ int piv[15], stop;
+  const int t = threadIdx.x;
+  // ---- the 34 sums: thread (group g, column k) adds rows g, g + G, ... with eight interleaved partial sums, then the groups in order
+  if (t < 34 * LIO_GROUPS) {
+    const int k = t % 34, g = t / 34;
+    double p0 = 0, p1 = 0, p2 = 0, p3 = 0, p4 = 0, p5 = 0, p6 = 0, p7 = 0;
+    int r = g;
+    for (; r + 7 * LIO_GROUPS < nrows; r += 8 * LIO_GROUPS) {
+      const double* q = rows + 34 * size_t(r) + k;
+      p0 += q[0]; p1 += q[34 * LIO_GROUPS]; p2 += q[68 * LIO_GROUPS]; p3 += q[102 * LIO_GROUPS];
+      p4 += q[136 * LIO_GROUPS]; p5 += q[170 * LIO_GROUPS]; p6 += q[204 * LIO_GROUPS]; p7 += q[238 * LIO_GROUPS];
+    }
+    for (; r < nrows; r += LIO_GROUPS) p0 += rows[34 * size_t(r) + k];
+    red[g][k] = ((p0 + p1) + (p2 + p3)) + ((p4 + p5) + (p6 + p7));
+  }
+  __syncthreads();
+  if (t < 34) {
+    double v = red[0][t];
+    for (int g = 1; g < LIO_GROUPS; g++) v += red[g][t];
+    sum[t] = v;
+  }
+  __syncthreads();
+  if (t < 36) {   // HTH from its upper triangle (row-major 21)
+    const int i = t / 6, j = t % 6, lo = i < j ? i : j, hi = i < j ? j : i;
+    HTH[i][j] = sum[lo * 6 - lo * (lo - 1) / 2 + (hi - lo)];
+  }
+  __syncthreads();
+  // ---- K_1 = (H_T_H + cov_inv)^-1,  H_T_H.block<6,6>(0,0) = HTH  (:920-921)
+  if (t < 225) { const int i = t / 15, j = t % 15; a[i][j] = (i < 6 && j < 6) ? ladd(HTH[i][j], s->cov_inv[t]) : s->cov_inv[t]; }
+  __syncthreads();
+  if (!lio_inverse15(a, K1, piv)) { if (t == 0) { s->err = 1; s->stopped = 1; } return; }
+  // ---- G.block<15,6> = K_1.block<15,6> HTH;  vec = x_prop - x_curr (IMUST::operator-, tools.hpp:164-173)
+  if (t < 90) {
+    const int i = t / 6, c = t % 6;
+    double v = lmul(K1[i][0], HTH[0][c]);
+    for (int k = 1; k < 6; k++) v = ladd(v, lmul(K1[i][k], HTH[k][c]));
+    G[i][c] = v;
+  } else if (t == 96) {
+    const double* R = s->x; const double* Rp = s->xp;
+    double D[9];
+    for (int i = 0; i < 3; i++)
+      for (int j = 0; j < 3; j++) { double v = lmul(R[i], Rp[j]); for (int k = 1; k < 3; k++) v = ladd(v, lmul(R[3 * k + i], Rp[3 * k + j])); D[3 * i + j] = v; }   // x.R^T xp.R
+    lio_log(D, vec);
+    for (int k = 3; k < 15; k++) vec[k] = lsub(s->xp[6 + k], s->x[6 + k]);
+  }
+  __syncthreads();
+  // ---- solution = K_1.block<15,6> HTz + vec - G.block<15,6> vec.head(6)  (:923)
+  if (t < 15) {
+    double u = lmul(K1[t][0], sum[21]), w = lmul(G[t][0], vec[0]);
+    for (int k = 1; k < 6; k++) { u = ladd(u, lmul(K1[t][k], sum[21 + k])); w = ladd(w, lmul(G[t][k], vec[k])); }
+    sol[t] = lsub(ladd(u, vec[t]), w);
+  }
+  __syncthreads();
+  // ---- x_curr += solution (IMUST::operator+=, tools.hpp:154-162), the convergence test, rematch_num and the stop rule (:925-946)
+  if (t == 0) {
+    double E[9], R[9];
+    lio_exp(sol, E);
+    for (int i = 0; i < 3; i++)
+      for (int j = 0; j < 3; j++) { double v = lmul(s->x[3 * i], E[j]); for (int k = 1; k < 3; k++) v = ladd(v, lmul(s->x[3 * i + k], E[3 * k + j])); R[3 * i + j] = v; }
+    for (int k = 0; k < 9; k++) s->x[k] = R[k];
+    for (int k = 3; k < 15; k++) s->x[6 + k] = ladd(s->x[6 + k], sol[k]);
+    const double rn = sqrt(ladd(ladd(lmul(sol[0], sol[0]), lmul(sol[1], sol[1])), lmul(sol[2], sol[2])));
+    const double tn = sqrt(ladd(ladd(lmul(sol[3], sol[3]), lmul(sol[4], sol[4])), lmul(sol[5], sol[5])));
+    const int it = s->iters;
+    const bool converged = lmul(rn, 57.3) < 0.01 && lmul(tn, 100.0) < 0.015;
+    if (converged || (s->rematch == 0 && it == 4 - 2)) s->rematch++;
+    stop = s->rematch >= 2 || it == 4 - 1;
+    s->trace[3 * it] = sum[33]; s->trace[3 * it + 1] = rn; s->trace[3 * it + 2] = tn;
+    s->match_num = sum[33];
+    s->iters = it + 1;
+    for (int k = 0; k < 12; k++) s->st[k] = s->x[k];       // R, p for the next pass; rot_var / tsl_var stay
+  }
+  __syncthreads();
+  if (!stop) return;
+  // ---- the stop: x_curr.cov = (I - G) x_curr.cov (:944), then the smallest eigenvalue of this iteration's nnt (:950-956)
+  if (t < 225) {
+    const int i = t / 15, j = t % 15;
+    double v = 0.0;
+    for (int k = 0; k < 15; k++) {
+      const double m = k < 6 ? lsub(i == k ? 1.0 : 0.0, G[i][k]) : (i == k ? 1.0 : 0.0);   // (I - G)(i, k); G is zero beyond column 5
+      v = k ? ladd(v, lmul(m, s->cov[15 * k + j])) : lmul(m, s->cov[j]);
+    }
+    ncov[t] = v;
+  }
+  __syncthreads();
+  if (t < 225) s->cov[t] = ncov[t];
+  if (t == 0) {
+    sym3 C; C.xx = sum[27]; C.xy = sum[28]; C.xz = sum[29]; C.yy = sum[30]; C.yz = sum[31]; C.zz = sum[32];
+    double w[3]; d3 u0, u1, u2;
+    eig3_jacobi(C, w, u0, u1, u2);
+    s->ok = !(w[0] < 14);
+    s->stopped = 1;
+  }
+}
+
 OdomScratch* odom_scratch(vxs_ctx* c) { if (!c->odom_scratch) c->odom_scratch = new OdomScratch(); return static_cast<OdomScratch*>(c->odom_scratch); }
 
 }  // namespace
@@ -185,7 +383,7 @@ OdomScratch* odom_scratch(vxs_ctx* c) { if (!c->odom_scratch) c->odom_scratch = 
 void vxs_odom_release(vxs_ctx* c) {
   if (!c->odom_scratch) return;
   OdomScratch* s = static_cast<OdomScratch*>(c->odom_scratch);
-  s->keys.release(); s->rows.release(); s->pts.release(); s->out.release(); s->st.release(); s->flags.release();
+  s->keys.release(); s->rows.release(); s->pts.release(); s->out.release(); s->st.release(); s->flags.release(); s->lio.release(); s->parts.release();
   delete s;
   c->odom_scratch = nullptr;
 }
@@ -271,8 +469,8 @@ extern "C" int vxs_odom_accumulate(vxs_ctx* ctx, const double* pv12, int64_t n, 
   int* dflags = nullptr;
   if (flags) { VXS_CUDA(ctx, s->flags.reserve(size_t(std::max<int64_t>(n, 1)))); dflags = s->flags.p; }
   if (n > 0 && s->n_planes > 0)
-    VXS_LAUNCH(ctx, "k_odom_accumulate", k_odom_accumulate, unsigned((n + 255) / 256), 256, 0, s->pts.p, (long long)n, s->st.p, s->keys.p, s->rows.p, s->n_planes, s->minx, s->miny, s->minz,
-               s->ex, s->ey, s->ez, s->voxel_size, s->max_layer, s->out.p, dflags);
+    VXS_LAUNCH(ctx, "k_odom_accumulate", k_odom_accumulate<false>, unsigned((n + 255) / 256), 256, 0, s->pts.p, (long long)n, s->st.p, s->keys.p, s->rows.p, s->n_planes, s->minx, s->miny,
+               s->minz, s->ex, s->ey, s->ez, s->voxel_size, s->max_layer, s->out.p, dflags, nullptr);
   else if (flags && n > 0) VXS_CUDA(ctx, cudaMemsetAsync(dflags, 0, size_t(n) * 4, ctx->stream));
   double out[34];
   VXS_CUDA(ctx, cudaMemcpyAsync(out, s->out.p, sizeof out, cudaMemcpyDeviceToHost, ctx->stream));
@@ -344,4 +542,56 @@ extern "C" int vxs_pvec_update(vxs_ctx* ctx, const double* pv12, int64_t n, cons
   if (pwld_out) VXS_CUDA(ctx, cudaMemcpyAsync(pwld_out, pw, size_t(n) * 24, cudaMemcpyDeviceToHost, ctx->stream));
   VXS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return VXS_OK;
+}
+
+// ---------------------------------------------------------------- lio_state_estimation on the device (voxelslam.cpp:856-958)
+// Enqueued without a host round trip: cov_inv, then 4 x (association pass, step) unconditionally; the step that stops sets the stopped flag and
+// every later launch returns at entry.  One read-back and one synchronisation per call.
+int vxs_lio_run(vxs_ctx* ctx, const char* who, const double* pv12, int64_t n, bool has_map, const vxs_lio_assoc& assoc, double* state24, double* cov225, int32_t* ok,
+                int32_t* iters, int64_t* match_num, double* trace12, int32_t* flags) {
+  cudaSetDevice(ctx->device);
+  OdomScratch* s = odom_scratch(ctx);
+  if (pv12) { int rc = vxs_odom_set_resident_scan(ctx, pv12, n); if (rc) return rc; }
+  else if (n != s->n_pts) return vxs_fail(ctx, VXS_ERR_ARG, (std::string(who) + ": no resident scan of this size").c_str());
+  LioState h;
+  std::memset(&h, 0, sizeof h);
+  for (int k = 0; k < 12; k++) h.st[k] = state24[k];
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) { h.st[12 + 3 * i + j] = cov225[15 * i + j]; h.st[21 + 3 * i + j] = cov225[15 * (3 + i) + 3 + j]; }
+  for (int k = 0; k < 24; k++) h.x[k] = h.xp[k] = state24[k];
+  for (int k = 0; k < 225; k++) h.cov[k] = cov225[k];
+  const unsigned grid = (n > 0 && has_map) ? unsigned((n + OD_THREADS - 1) / OD_THREADS) : 0u;
+  VXS_CUDA(ctx, s->lio.reserve((sizeof(LioState) + 7) / 8));
+  VXS_CUDA(ctx, s->parts.reserve(size_t(std::max(grid, 1u)) * 34));
+  int* dflags = nullptr;
+  if (flags && n > 0) { VXS_CUDA(ctx, s->flags.reserve(size_t(n))); dflags = s->flags.p; }
+  LioState* d = reinterpret_cast<LioState*>(s->lio.p);
+  VXS_CUDA(ctx, cudaMemcpyAsync(d, &h, sizeof h, cudaMemcpyHostToDevice, ctx->stream));
+  if (dflags && !grid) VXS_CUDA(ctx, cudaMemsetAsync(dflags, 0, size_t(n) * 4, ctx->stream));
+  VXS_LAUNCH(ctx, "k_lio_init", k_lio_init, 1, LIO_THREADS, 0, d);
+  for (int it = 0; it < 4; it++) {
+    if (grid) { int rc = assoc(grid, s->pts.p, (long long)n, d->st, &d->stopped, s->parts.p, dflags); if (rc) return rc; }
+    VXS_LAUNCH(ctx, "k_lio_step", k_lio_step, 1, LIO_THREADS, 0, d, s->parts.p, int(grid));
+  }
+  VXS_CUDA(ctx, cudaMemcpyAsync(&h, d, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+  if (dflags) VXS_CUDA(ctx, cudaMemcpyAsync(flags, dflags, size_t(n) * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  VXS_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (h.err) return vxs_fail(ctx, VXS_ERR_ARG, (std::string(who) + ": exact zero pivot in the inverse of the covariance").c_str());
+  for (int k = 0; k < 24; k++) state24[k] = h.x[k];
+  for (int k = 0; k < 225; k++) cov225[k] = h.cov[k];
+  *ok = h.ok; *iters = h.iters; *match_num = int64_t(h.match_num);
+  if (trace12) for (int k = 0; k < 12; k++) trace12[k] = h.trace[k];
+  return VXS_OK;
+}
+
+extern "C" int vxs_odom_lio_update(vxs_ctx* ctx, const double* pv12, int64_t n, double* state24, double* cov225, int32_t* ok, int32_t* iters, int64_t* match_num, double* trace12,
+                                   int32_t* flags) {
+  if (!ctx || n < 0 || !state24 || !cov225 || !ok || !iters || !match_num) return VXS_ERR_ARG;
+  OdomScratch* s = odom_scratch(ctx);
+  auto assoc = [&](unsigned grid, const double* pv, long long np, const double* st, const int* stopped, double* rows, int* fl) -> int {
+    VXS_LAUNCH(ctx, "k_odom_accumulate_rows", k_odom_accumulate<true>, grid, OD_THREADS, 0, pv, np, st, s->keys.p, s->rows.p, s->n_planes, s->minx, s->miny, s->minz, s->ex, s->ey,
+               s->ez, s->voxel_size, s->max_layer, rows, fl, stopped);
+    return VXS_OK;
+  };
+  return vxs_lio_run(ctx, "vxs_odom_lio_update", pv12, n, s->n_planes > 0, assoc, state24, cov225, ok, iters, match_num, trace12, flags);
 }

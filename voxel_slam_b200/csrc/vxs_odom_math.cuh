@@ -63,3 +63,24 @@ __device__ __forceinline__ void od_flush(const double* acc, double* __restrict__
     if ((threadIdx.x & 31) == 0 && v != 0.0) atomicAdd(out + k, v);
   }
 }
+// The same 34 sums without atomics, for the iterated EKF update whose branches they decide: the warp tree above, then the warps of the
+// block in ascending order through shared memory, one partial row per block (row = out + 34 * blockIdx.x).  Bit-reproducible for a fixed
+// grid.  Every thread of the block must reach it; blockDim.x == OD_THREADS.
+#define OD_THREADS 256
+__device__ __forceinline__ void od_flush_row(const double* acc, double* __restrict__ out) {
+  __shared__ double red[OD_THREADS / 32][34];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 34; k++) {
+    double v = acc[k];
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
+    if (lane == 0) red[w][k] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < 34) {
+    double s = red[0][threadIdx.x];
+#pragma unroll
+    for (int j = 1; j < OD_THREADS / 32; j++) s += red[j][threadIdx.x];
+    out[34 * size_t(blockIdx.x) + threadIdx.x] = s;
+  }
+}
